@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the RenderIH hot path on B200.
+"""Benchmark of the RenderIH hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            # ours: BASELINE.json configs[2] (the headline metric)
     python bench.py --impl reference ...                     # the UNMODIFIED reference's own CPU path on the host cores
@@ -10,7 +10,7 @@ Default = images/sec of one training step (forward + calc_loss_GCN + backward + 
 GPU, 256x256 synthetic images.  Prints ONE JSON line on rank 0 (contract in the task statement):
   value               device-timed images/s with inputs resident in HBM
   e2e                 the same step through the public TrainStep API from pinned HOST buffers (image + labels H2D every step, loss D2H)
-  roofline            the kernel CLASS with the largest share of the step (all tcgen05 GEMM / implicit-GEMM launches), each launch
+  roofline            the kernel CLASS with the largest share of the step (all wgmma GEMM / implicit-GEMM launches), each launch
                       bracketed by CUDA events on its own stream during one eager step; + `step`: whole-step achieved / peak
   roofline_top_kernel the single most expensive launch timed alone (+ DRAM traffic from the committed ncu capture)
   gpu_eager_baseline  the UNMODIFIED reference graph `.cuda()` in eager PyTorch on the same GPU (north_star's comparator) and the
@@ -61,10 +61,31 @@ def parse():
     ap.add_argument('--skip-cpu-baseline', action='store_true')
     ap.add_argument('--skip-gpu-eager', action='store_true', help='do not time the reference graph in eager PyTorch on this GPU')
     ap.add_argument('--gpu-eager-iters', type=int, default=100, help='timed iterations of the GPU eager baseline (SURVEY 8d: 20 warm-up + 100)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last step computed as DIR/<name>.npy (float32 / float64, at most 64 MB in all; '
+                         'large outputs as a fixed seeded sample) so that two builds can be compared output for output')
     a = ap.parse_args()
     if a.batch is None:
         a.batch = 32 if a.encoder == 'hrnet48' else 64
     return a
+
+
+DUMP_LIMIT = 64 << 20       # bytes written by --dump-outputs in all
+
+
+def dump_outputs(path, arrays):
+    """arrays: {name: tensor or ndarray}.  Writes DIR/<name>.npy in float32 (float64 stays float64).  An array larger than its share of
+    DUMP_LIMIT is replaced by a fixed sample of its flattened elements (the same sorted indices in every run) and named <name>_sample."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    share = DUMP_LIMIT // max(1, len(arrays))
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if hasattr(a, 'detach') else np.asarray(a)
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        if a.nbytes > share:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, share // a.itemsize, replace=False))
+            a, name = a.reshape(-1)[idx], name + '_sample'
+        np.save(os.path.join(path, name + '.npy'), a)
 
 
 def peaks():
@@ -74,7 +95,7 @@ def peaks():
         return {'hbm_gbs': p['hbm_gbs'], 'tflops': p['bf16_tflops'], 'tflops_sustained': p.get('bf16_tflops_sustained', p['bf16_tflops']),
                 'src': 'measured (MEASURED_PEAKS.json)'}
     except Exception:
-        return {'hbm_gbs': 6650.0, 'tflops': 1590.0, 'tflops_sustained': 1400.0, 'src': 'fallback (B200_PROFILING.md)'}
+        return {'hbm_gbs': 3350.0, 'tflops': 989.0, 'tflops_sustained': 989.0, 'src': 'H100 SXM data sheet (dense BF16, 700 W card), not measured'}
 
 
 class ClockSampler:
@@ -342,7 +363,7 @@ def _gemm_flops(name, a):
 
 def class_roofline(torch, step, pk, flops_step, ms_step):
     """The dominant kernel CLASS of the step, measured live: during ONE eager (un-captured) step every C-ABI launch is bracketed by CUDA
-    events on the stream it is launched on (`_lib.TRACE`); the launches that run on the tcgen05 GEMM / implicit-GEMM kernels
+    events on the stream it is launched on (`_lib.TRACE`); the launches that run on the wgmma GEMM / implicit-GEMM kernels
     (nn.Linear, Conv2d and attention contractions: forward, dgrad, wgrad) form the class.  achieved = sum of their algorithmic flops /
     sum of their event-timed durations.  Event pairs around a short kernel include a few microseconds of launch gap, so this
     under-states the class a little; the share of the step is computed against the sum over ALL traced launches (serialised time)."""
@@ -385,7 +406,7 @@ def class_roofline(torch, step, pk, flops_step, ms_step):
                 out.append(v)
         return out
     slow = sorted(((e0.elapsed_time(e1), name, a) for name, a, e0, e1 in trace), key=lambda t: -t[0])[:16]
-    return {'bound': 'tensor', 'kernel': 'class: every tcgen05 GEMM / implicit-GEMM launch of the step (gemm_tc_persistent_kernel<...>: Conv2d, nn.Linear and attention '
+    return {'bound': 'tensor', 'kernel': 'class: every wgmma GEMM / implicit-GEMM launch of the step (gemm_tc_persistent_kernel<...>: Conv2d, nn.Linear and attention '
                                          'contractions, fwd + dgrad + wgrad), %d launches' % n,
             'achieved': ach, 'peak': peak, 'unit': 'TFLOP/s', 'frac': ach / peak, 'frac_of_tf32_peak': ach / (0.5 * peak), 'traffic': None,
             'share_of_step_kernel_time': cms / total_ms if total_ms else None, 'class_ms_per_step': cms, 'all_kernels_ms_per_step_serialised': total_ms,
@@ -393,7 +414,7 @@ def class_roofline(torch, step, pk, flops_step, ms_step):
             'how': 'one eager step, CUDA events around every C-ABI launch on its own stream (cold launch gaps included); ncu launch list of the same step: profiles/',
             'peak_source': pk['src'] + ' bf16 dense SUSTAINED (kernels timed inside a long step); operands are TF32, whose tensor peak is half of it',
             'by_entry_point_ms': {k: round(v[1], 3) for k, v in top},
-            'gemm_launches_by_path': {'tcgen05_tma_store_epilogue': counts[0], 'tcgen05_thread_store_epilogue': counts[1], 'exact_fp32_simt': counts[2]},
+            'gemm_launches_by_path': {'wgmma_tma_store_epilogue': counts[0], 'wgmma_thread_store_epilogue': counts[1], 'exact_fp32_simt': counts[2]},
             'slowest_calls': [{'ms': round(ms, 3), 'entry': name, 'int_args': small_ints(a)} for ms, name, a in slow],
             'step': {'achieved': flops_step / (ms_step * 1e-3) / 1e12, 'peak': peak, 'unit': 'TFLOP/s',
                      'frac': flops_step / (ms_step * 1e-3) / 1e12 / peak, 'frac_of_tf32_peak': flops_step / (ms_step * 1e-3) / 1e12 / (0.5 * peak),
@@ -609,7 +630,7 @@ def run_forward(args):
         graph.replay()
     sampler = ClockSampler(0)
     sampler.start()
-    steps = max(args.steps, 20)
+    steps = args.steps
     ms_dev = timed(lambda i: graph.replay(), steps)
 
     def e2e(i):
@@ -622,14 +643,16 @@ def run_forward(args):
         e2e(i)
     ms_e2e = timed(e2e, steps)
     clocks = sampler.stop()
+    if args.dump_outputs:                     # the last timed forward: what a caller reads back
+        dump_outputs(args.dump_outputs, {'verts3d_%s' % k: v for k, v in host_out.items()})
     pk = peaks()
     gf = FLOPS[args.encoder][1]
     value = B / (ms_dev * 1e-3)
     line = {'metric': metric_name(args), 'value': value, 'unit': 'images/s', 'n_gpus': 1, 'steps': steps, 'warmup': max(3, args.warmup),
             'ms_per_step': ms_dev, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
-            'dtype': 'f32 storage; tcgen05 TF32 convolutions + 3xTF32 Linear / attention GEMMs (--gemm-mode %s), fp32 accumulate' % args.gemm_mode, 'data': 'synthetic',
+            'dtype': 'f32 storage; wgmma TF32 convolutions + 3xTF32 Linear / attention GEMMs (--gemm-mode %s), fp32 accumulate' % args.gemm_mode, 'data': 'synthetic',
             'config': {'workload': workload_name(args.encoder, B, 'forward'), 'cuda_graph': True, 'algorithmic_gflop_per_image_fwd': gf / 1e9,
-                       'l2': 'per-step working set (activations, > 1 GB) >> 126 MB L2; no explicit flush needed'},
+                       'l2': 'per-step working set (activations, > 1 GB) >> 50 MB L2; no explicit flush needed'},
             'achieved_tflops': value * gf / 1e12,
             'roofline': {'bound': 'tensor', 'kernel': 'whole forward (encoder + attention/GCN decoder + heads): north_star\'s 70 %% target is stated on this',
                          'achieved': value * gf / 1e12, 'peak': pk['tflops_sustained'], 'unit': 'TFLOP/s', 'frac': value * gf / 1e12 / pk['tflops_sustained'],
@@ -743,6 +766,8 @@ def run_ours(args):
         e2e_step(i)
     ms_e2e = timed(e2e_step, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if rank == 0 and args.dump_outputs:       # the last timed step: its loss and the parameters it updated
+        dump_outputs(args.dump_outputs, {'loss': [losses[-1]], 'params': step.flatp.flat})
     exposed = None
     if world > 1:        # exposed communication = step time with the gradient exchange - step time without it (one extra timed pass on every rank)
         if getattr(step, 'overlap', False) and not args.no_graph:
@@ -764,13 +789,13 @@ def run_ours(args):
     roof_top = top_kernel_roofline(torch, B, pk, conv_mode)
     line = {'metric': metric_name(args),
             'value': value, 'unit': 'images/s', 'n_gpus': world, 'steps': args.steps, 'warmup': max(3, args.warmup), 'ms_per_step': ms_dev,
-            'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': {'simt': 'f32', 'refrn': 'f32 storage; tcgen05 TF32(rn) convolutions (cuDNN-default class of the reference) + 3xTF32 fp32-faithful Linear GEMMs, fp32 accumulate',
+            'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': {'simt': 'f32', 'refrn': 'f32 storage; wgmma TF32(rn) convolutions (cuDNN-default class of the reference) + 3xTF32 fp32-faithful Linear GEMMs, fp32 accumulate',
                       'tf32': 'tf32 (truncating) conv+Linear, fp32 accumulate/storage', 'tf32c': 'tf32 (truncating, mean-compensated) conv+Linear, fp32 accumulate/storage',
-                      'ref': 'f32 storage; tcgen05 TF32 convolutions (truncating + mean-compensated: the accuracy class of the reference\'s cuDNN-TF32 default, measured) + 3xTF32 fp32-faithful Linear GEMMs, fp32 accumulate', 'tf32rn': 'tf32 (rn) conv+Linear, fp32 accumulate/storage',
+                      'ref': 'f32 storage; wgmma TF32 convolutions (truncating + mean-compensated: the accuracy class of the reference\'s cuDNN-TF32 default, measured) + 3xTF32 fp32-faithful Linear GEMMs, fp32 accumulate', 'tf32rn': 'tf32 (rn) conv+Linear, fp32 accumulate/storage',
                       'tf32x3': '3xTF32 (fp32-faithful) conv+Linear, fp32 accumulate/storage'}[args.gemm_mode], 'data': 'synthetic',
             'config': {'workload': workload_name(args.encoder, B),
                        'global_batch': total_imgs, 'parallelism': 'dp%d' % world, 'cuda_graph': not args.no_graph,
-                       'l2': 'per-step working set (activations, several GB) >> 126 MB L2; no explicit flush needed',
+                       'l2': 'per-step working set (activations, several GB) >> 50 MB L2; no explicit flush needed',
                        'algorithmic_gflop_per_image': flops_fb / 1e9},
             'achieved_tflops': value * flops_fb / 1e12 / world,
             'e2e': {'value': e2e, 'unit': 'images/s', 'ms_per_step': ms_e2e, 'h2d_bytes_per_step': h2d, 'd2h_bytes_per_step': 4,

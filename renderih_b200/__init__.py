@@ -1,4 +1,4 @@
-"""renderih_b200 -- B200-native (sm_100a) hot path of adwardlee/RenderIH: HandNET_GCN forward/backward + ManoLayer.
+"""renderih_b200 -- H100-native (sm_90a) hot path of adwardlee/RenderIH: HandNET_GCN forward/backward + ManoLayer.
 
 Public API mirrors the reference modules it replaces:
     load_model(cfg) / HandNET_GCN      <-  models/model.py:18-60
@@ -16,7 +16,7 @@ from . import _build
 
 
 def build(force=False):
-    """Compile the CUDA library for sm_100a (in-tree)."""
+    """Compile the CUDA library for sm_90a (in-tree)."""
     return _build.build(force=force)
 
 

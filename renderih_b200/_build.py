@@ -1,4 +1,4 @@
-"""In-tree build of the C-ABI CUDA library (sm_100a only).  `python -m renderih_b200._build` or `build()`.
+"""In-tree build of the C-ABI CUDA library (sm_90a only).  `python -m renderih_b200._build` or `build()`.
 
 The shared object is written next to this file (`renderih_b200/librih_b200.so`): it is git-ignored
 but travels to the GPU box with the gpurun snapshot.  nvcc cross-compiles without a GPU.
@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB_PATH = os.path.join(HERE, 'librih_b200.so')
 STAMP_PATH = os.path.join(HERE, 'csrc', '.build_stamp')
-ARCH_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a']
 
 
 def _sources():

@@ -185,7 +185,7 @@ RIH_API int rih_attn_fwd(const float* q, long long q_bs, int ldq, const float* k
   size_t smem = sizeof(float) * (2 * (size_t)Skr * (d + 4) + ATT_WARPS * RF * d + (size_t)ATT_WARPS * RF * Skr);
   RIH_REQUIRE(smem <= 227 * 1024, "attn_fwd: shared memory %zu too large", smem);
   int ysplit = 1;
-  while (B * H * ysplit < 148 * 2 && Sq / (ysplit * 2) >= 32) ysplit *= 2;
+  while (B * H * ysplit < sm_count() * 2 && Sq / (ysplit * 2) >= 32) ysplit *= 2;
   int rows_per_cta = cdiv(Sq, ysplit);
   rows_per_cta = (rows_per_cta + RF - 1) / RF * RF;
   dim3 grid(B * H, cdiv(Sq, rows_per_cta));
@@ -434,7 +434,7 @@ RIH_API int rih_attn_set_row_blocks(int rows_fwd, int rows_bwd) {
 }
 
 // ================================================================================================ tensor-core attention core
-// The same operator with its four contractions on the tcgen05 tensor cores (TMA -> shared memory -> tcgen05.mma, 3xTF32 or TF32), as
+// The same operator with its four contractions on the wgmma tensor cores (TMA -> shared memory -> wgmma, 3xTF32 or TF32), as
 // batched per-head GEMMs over 4-D tensor maps (gemm_tc.cu: bgemm_tf32) around two warp-per-row softmax kernels:
 //   forward : S = scale * Q K^T  ->  P = softmax(S), P~ = dropout(P)  ->  O = P~ V
 //   backward: dP~ = dO V^T  ->  dS = P o (dP~ o M - rowsum(dP~ o M o P)), P~ = P o M  ->  dQ = scale dS K, dK = scale dS^T Q, dV = P~^T dO

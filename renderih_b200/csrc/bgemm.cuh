@@ -1,4 +1,4 @@
-// Batched per-head GEMM of the attention core on the tcgen05 path (implemented in gemm_tc.cu, used by attention.cu).
+// Batched per-head GEMM of the attention core on the wgmma path (implemented in gemm_tc.cu, used by attention.cu).
 #pragma once
 #include <cuda_runtime.h>
 

@@ -32,8 +32,21 @@ int stream_cta_limit(cudaStream_t s, int num_sms) {
 }
 int g_ew_cap = 1;
 long long ew_ctas(cudaStream_t s) {
-  if (g_ew_cap) for (int i = 0; i < CAP_SLOTS; ++i) if (g_cap_ctas[i] > 0 && g_cap_stream[i] == s && g_cap_ctas[i] < 96) return 148 * 4;
-  return 148 * 16;
+  if (g_ew_cap) for (int i = 0; i < CAP_SLOTS; ++i) if (g_cap_ctas[i] > 0 && g_cap_stream[i] == s && 3 * g_cap_ctas[i] < 2 * sm_count()) return sm_count() * 4;
+  return sm_count() * 16;
+}
+
+// SMs of the current device (132 on an H100 SXM), queried once per device
+int sm_count() {
+  static int n[64] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
+  if (!n[dev]) {
+    int v = 0;
+    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+    n[dev] = v > 0 ? v : 132;
+  }
+  return n[dev];
 }
 
 int check_launch(const char* what) {
@@ -55,7 +68,7 @@ RIH_API int rih_set_pdl(int on) { rih::g_pdl = on ? 1 : 0; return 0; }
 
 // Traversal direction of the NEXT launches: 1 = the tensor-core GEMM / convolution kernels walk their output tiles, and the BatchNorm passes
 // their rows, from the last to the first.  A consumer that starts where its producer finished finds the most recently written part of an
-// activation (whatever of it fits in the 126 MB L2) still cached; alternating the direction kernel by kernel ("serpentine") keeps that true
+// activation (whatever of it fits in the 50 MB L2) still cached; alternating the direction kernel by kernel ("serpentine") keeps that true
 // along a whole chain of layers.  Scheduling only: results are unchanged up to summation order in atomically accumulated statistics.
 RIH_API int rih_set_traversal(int reverse) { rih::g_reverse = reverse ? 1 : 0; return 0; }
 
@@ -70,7 +83,7 @@ RIH_API int rih_set_ew_cap(int on) { rih::g_ew_cap = on ? 1 : 0; return 0; }
 
 RIH_API int rih_set_l2_hints(int on) { rih::g_l2_hints = on ? 1 : 0; return 0; }
 
-// Device properties probe (used by the host side to fail loudly on a non-sm_100 device).
+// Device properties probe (used by the host side to fail loudly on a device other than sm_90).
 RIH_API int rih_device_info(int device, int* cc_major, int* cc_minor, int* sm_count, size_t* smem_optin) {
   cudaDeviceProp p;
   RIH_CUDA(cudaGetDeviceProperties(&p, device));

@@ -1,4 +1,4 @@
-// Common helpers for the renderih_b200 C-ABI CUDA library (sm_100a only).
+// Common helpers for the renderih_b200 C-ABI CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -14,7 +14,8 @@ void set_error(const char* fmt, ...);
 int check_launch(const char* what);
 int set_stream_cta_limit(cudaStream_t s, int ctas);
 int stream_cta_limit(cudaStream_t s, int num_sms);
-long long ew_ctas(cudaStream_t s);      // grid cap of element-wise kernels on stream s (148 * 16, or 148 * 4 on a CTA-capped stream)
+long long ew_ctas(cudaStream_t s);      // grid cap of element-wise kernels on stream s (16 per SM, or 4 per SM on a CTA-capped stream)
+int sm_count();                         // SMs of the current device
 
 #define RIH_REQUIRE(cond, ...)                        \
   do {                                                \
@@ -39,7 +40,7 @@ static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b)
 // Every kernel of this library is launched through launch_k() and starts with pdl_sync() (or its two halves).  With g_pdl != 0 the launch
 // carries cudaLaunchAttributeProgrammaticStreamSerialization: the kernel may be scheduled as soon as every CTA of its stream predecessor has
 // executed griddepcontrol.launch_dependents (first instruction of all our kernels) -- its CTAs become resident on free SMs, run their
-// prologue (barrier init, TMEM allocation, tensor-map prefetch) and then block in griddepcontrol.wait until the predecessor has COMPLETED and
+// prologue (barrier init, tensor-map prefetch) and then block in griddepcontrol.wait until the predecessor has COMPLETED and
 // its memory operations are visible.  That takes the launch latency and the prologue off the dependent chains of the decoder (hundreds of
 // 5-15 us kernels).  Nothing before pdl_wait() may touch global memory a predecessor writes.  Under CUDA-graph capture the edges become
 // programmatic dependencies of the graph.  g_pdl == 0: plain launches; griddepcontrol.* are no-ops then.

@@ -28,9 +28,9 @@ int stem_fwd_tf32(const float* xp, const float* w224, Epilogue ep, int N, int H,
 int stem_wgrad_tf32(const float* dy, int lddy, const float* xp, Epilogue ep, int N, int H, int W, cudaStream_t s);
 } }
 
-// Arithmetic mode of the GEMM-class ops: 0 = SIMT fp32 (exact), 1 = tcgen05 TF32 multiplicands / fp32 accumulate,
-// 2 = tcgen05 3xTF32 (hi/lo split in shared memory, fp32-faithful), 3 = tcgen05 TF32 with round-to-nearest operand
-// conversion in shared memory (single MMA pass, unbiased -- the cuDNN / cuBLAS TF32 convention), 4 = tcgen05 TF32 with the
+// Arithmetic mode of the GEMM-class ops: 0 = SIMT fp32 (exact), 1 = wgmma TF32 multiplicands / fp32 accumulate,
+// 2 = wgmma 3xTF32 (hi/lo split in shared memory, fp32-faithful), 3 = wgmma TF32 with round-to-nearest operand
+// conversion in shared memory (single MMA pass, unbiased -- the cuDNN / cuBLAS TF32 convention), 4 = wgmma TF32 with the
 // hardware's truncating conversion and the accumulator multiplied by 1 + 7.05e-4 in the epilogue: truncation of a fp32
 // operand to TF32 shrinks it by 2^-11 * E[1/m] (m = mantissa in [1,2), E[1/m] = 0.72 under Benford's law) on average, so the
 // product of two truncated operands is low by 7.05e-4; removing that mean leaves the same error variance as rounding to
@@ -161,7 +161,7 @@ RIH_API int rih_conv2d_workspace(const int* geom, int which, long long* floats) 
   return 0;
 }
 
-// *supported = 1 when convolution pass `which` (0 fwd, 1 dgrad, 2 wgrad) of this geometry runs on the tcgen05 implicit-GEMM path in the
+// *supported = 1 when convolution pass `which` (0 fwd, 1 dgrad, 2 wgrad) of this geometry runs on the wgmma implicit-GEMM path in the
 // current gemm mode (1x1 / stride-1 / pad-0 convolutions are dense GEMMs and always do), 0 when it takes the exact-fp32 SIMT path.
 RIH_API int rih_conv2d_tc_supported(const int* geom, int which, int* supported) {
   ConvGeom g;
@@ -277,7 +277,7 @@ RIH_API int rih_conv2d_wgrad(const float* dy, const float* x, float* dw, const i
   return launch_gemm_simt(a, b, ep, g.Cout, Kn, (int)P, 1, stream, "conv2d_wgrad");
 }
 
-// RGB stem conv1 (7x7 / stride 2 / pad 3, 3 -> 64; torchvision resnet.conv1 as used by models/encoder.py:108) as a tcgen05 implicit GEMM
+// RGB stem conv1 (7x7 / stride 2 / pad 3, 3 -> 64; torchvision resnet.conv1 as used by models/encoder.py:108) as a wgmma implicit GEMM
 // over the zero-bordered NHWC4 image xp[N][H+6][W+8][4] written by rih_nchw_to_nhwc4_pad; w224 = the filter repacked as [64][7][8][4]
 // (8th column and 4th channel zero).  Tensor-core convolution modes only (rih_set_gemm_mode); `stats` as in rih_conv2d_fwd.
 RIH_API int rih_stem_conv_fwd(const float* xp, const float* w224, float* y, int N, int H, int W, double* stats, cudaStream_t stream) {

@@ -1,6 +1,6 @@
 // SIMT fp32 tiled GEMM core with pluggable operand loaders (dense / implicit-conv gathers).
 //   C[m,n] (+)= sum_k A(m,k) * B(n,k)
-// This is the exact-fp32 path (parity reference mode + shapes the tcgen05 path does not take).
+// This is the exact-fp32 path (parity reference mode + shapes the wgmma path does not take).
 #pragma once
 #include "common.cuh"
 

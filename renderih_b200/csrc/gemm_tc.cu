@@ -1,4 +1,4 @@
-// Host launchers + C-ABI for the tcgen05 TF32 GEMM / implicit-GEMM convolution (see gemm_tc.cuh).
+// Host launchers + C-ABI for the wgmma TF32 GEMM / implicit-GEMM convolution (see gemm_tc.cuh).
 #include "gemm_tc.cuh"
 #include "bgemm.cuh"
 
@@ -28,7 +28,7 @@ int make_tmap_2d(CUtensorMap* map, const float* base, long long rows, long long 
   CUresult r = CUDA_SUCCESS;
   for (int attempt = 0; attempt < 2; ++attempt) {
     r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-           CU_TENSOR_MAP_INTERLEAVE_NONE, atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_ERROR_INVALID_CONTEXT) break;
     cudaFree(0);   // this thread (e.g. an autograd worker) has no driver context bound yet: let the runtime bind the primary one
@@ -48,7 +48,7 @@ int make_tmap_2d_grouped(CUtensorMap* map, const float* base, long long rows, lo
   CUresult r = CUDA_SUCCESS;
   for (int attempt = 0; attempt < 2; ++attempt) {
     r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_ERROR_INVALID_CONTEXT) break;
     cudaFree(0);
   }
@@ -69,7 +69,7 @@ int make_tmap_nhwc(CUtensorMap* map, const float* base, int N, int H, int W, int
   CUresult r = CUDA_SUCCESS;
   for (int attempt = 0; attempt < 2; ++attempt) {
     r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), dims, strides, box, estr,
-           CU_TENSOR_MAP_INTERLEAVE_NONE, atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_ERROR_INVALID_CONTEXT) break;
     cudaFree(0);
@@ -90,7 +90,7 @@ int make_tmap_nhwc_grouped(CUtensorMap* map, const float* base, int N, int H, in
   CUresult r = CUDA_SUCCESS;
   for (int attempt = 0; attempt < 2; ++attempt) {
     r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<float*>(base), dims, strides, box, estr,
-           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_ERROR_INVALID_CONTEXT) break;
     cudaFree(0);
   }
@@ -109,7 +109,7 @@ int make_tmap_stem(CUtensorMap* map, const float* base, int N, int Hp, int Wp, i
   CUresult r = CUDA_SUCCESS;
   for (int attempt = 0; attempt < 2; ++attempt) {
     r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_ERROR_INVALID_CONTEXT) break;
     cudaFree(0);
   }
@@ -138,10 +138,8 @@ int make_tmap_wgrad_out(CUtensorMap* map, const float* base, int Cout, int taps,
 }
 
 int g_stats_fused = 0;            // set by the launcher when the epilogue accumulated ep.stats (fused BatchNorm statistics)
-static int g_wide_tiles = 1;     // 128 x 256 output tiles when N % 256 == 0
-void set_wide_tiles(int on) { g_wide_tiles = on ? 1 : 0; }
-static int g_wgrad_wide = 3;     // 256-wide multi-tap N tiles for the convolution weight gradients, also over padded channel counts (rih_set_wgrad_wide)
-void set_wgrad_wide(int on) { g_wgrad_wide = on & 3; }     // bit 0: multi-tap 256-wide tiles, bit 1: also for channel counts that are not multiples of 32
+static int g_wgrad_wide = 3;     // multi-tap N tiles for the convolution weight gradients, also over padded channel counts (rih_set_wgrad_wide)
+void set_wgrad_wide(int on) { g_wgrad_wide = on & 3; }     // bit 0: multi-tap 128-wide tiles, bit 1: also for channel counts that are not multiples of 32
 static int g_narrow_small = 1;   // 64-wide N tiles for GEMMs whose 128-wide tiling would leave half of the SMs idle (RIH_NARROW_TILES=0 to compare)
 void set_narrow_small(int on) { g_narrow_small = on ? 1 : 0; }
 static int g_persistent = 1;     // 0 = one CTA per tile (non-persistent kernel; debug / comparison)
@@ -158,20 +156,10 @@ void set_tma_res(int on) { g_tma_res = on ? 1 : 0; }
 template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT>
 static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep, const Producer& prod, int M, int N, int num_kb, int splits,
                       int kb_per_split, cudaStream_t s, const CUtensorMap* c_map = nullptr) {
-  auto kern = gemm_tc_kernel<BN, A_MN, B_MN, Producer, NSPLIT>;
-  static bool attr = false;
-  if (!attr) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<BN, NSPLIT>()) != cudaSuccess) {
-      set_error("gemm_tc: cannot raise dynamic shared memory to %d", smem_bytes<BN, NSPLIT>());
-      return 2;
-    }
-    attr = true;
-  }
-  dim3 grid(cdiv(N, BN), cdiv(M, BM), splits);
   // TMA-store epilogue whenever the output is a 16-byte aligned matrix (a residual is read back row-wise by the epilogue threads when it is aligned too)
   CUtensorMap tc_;
   int tma_epi = 0;
-  if (c_map) {       // caller-built output map (3-D wgrad view); only the persistent TMA-store epilogue understands it
+  if (c_map) {       // caller-built output map (3-D wgrad view, batched heads); only the persistent TMA-store epilogue understands it
     if (!g_persistent) { set_error("gemm_tc: output-map override needs the persistent kernel"); return 1; }
     tc_ = *c_map;
     tma_epi = 1;
@@ -184,30 +172,25 @@ static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep,
   }
   if (ep.col_scale && ep.bias) { set_error("gemm_tc: a folded per-column affine and a bias cannot be combined (fold the bias into the shift)"); return 1; }
   g_launch_counts[tma_epi ? 0 : 1]++;
-  if (g_persistent) {
-    auto pk = gemm_tc_persistent_kernel<BN, A_MN, B_MN, Producer, NSPLIT>;
-    static bool pattr = false;
-    if (!pattr) {
-      if (cudaFuncSetAttribute(pk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<BN, NSPLIT>()) != cudaSuccess) {
-        set_error("gemm_tc(persistent): cannot raise dynamic shared memory to %d", smem_bytes<BN, NSPLIT>());
-        return 2;
-      }
-      pattr = true;
+  auto pk = gemm_tc_persistent_kernel<BN, A_MN, B_MN, Producer, NSPLIT>;
+  static bool pattr = false;
+  if (!pattr) {
+    if (cudaFuncSetAttribute(pk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<BN, NSPLIT>()) != cudaSuccess) {
+      set_error("gemm_tc: cannot raise dynamic shared memory to %d", smem_bytes<BN, NSPLIT>());
+      return 2;
     }
-    static int num_sms = 0;
-    if (!num_sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev); if (num_sms <= 0) num_sms = 148; }
-    const int tiles_n = cdiv(N, BN), tiles_m = cdiv(M, BM);
-    const long long total = (long long)tiles_n * tiles_m * splits;
-    const int cap = stream_cta_limit(s, num_sms);
-    const int ctas = (int)(total < cap ? total : cap);
-    if (ep.stats && !(tma_epi && splits == 1)) ep.stats = nullptr;
-    g_stats_fused = ep.stats != nullptr;
-    launch_k(pk, dim3(ctas), dim3(persistent_threads<NSPLIT>()), (size_t)smem_bytes<BN, NSPLIT>(), s, ta, tb, tc_, ep, prod, num_kb, kb_per_split, tiles_m, tiles_n, splits, tma_epi);
-    return check_launch("gemm_tc_persistent");
+    pattr = true;
   }
-  g_stats_fused = 0;
-  launch_k(kern, grid, dim3(THREADS), (size_t)smem_bytes<BN, NSPLIT>(), s, ta, tb, tc_, ep, prod, num_kb, kb_per_split, tma_epi);
-  return check_launch("gemm_tc");
+  const int tiles_n = cdiv(N, BN), tiles_m = cdiv(M, BM);
+  const long long total = (long long)tiles_n * tiles_m * splits;
+  // persistent: at most one CTA per SM (fewer on a CTA-capped stream); otherwise one CTA per tile
+  const long long cap = g_persistent ? stream_cta_limit(s, sm_count()) : total;
+  const int ctas = (int)(total < cap ? total : cap);
+  if (ep.stats && !(g_persistent && tma_epi && splits == 1)) ep.stats = nullptr;
+  g_stats_fused = ep.stats != nullptr;
+  launch_k(pk, dim3(ctas), dim3(persistent_threads<A_MN, B_MN, NSPLIT>()), (size_t)smem_bytes<BN, NSPLIT>(), s, ta, tb, tc_, ep, prod, num_kb, kb_per_split,
+           tiles_m, tiles_n, splits, tma_epi);
+  return check_launch(g_persistent ? "gemm_tc_persistent" : "gemm_tc");
 }
 static int g_nsplit = 1;   // set per call by the dispatchers below (1 = TF32, 2 = TF32 rn, 3 = 3xTF32)
 static float g_scale = 1.f; // accumulator scale (bias-compensated truncating TF32)
@@ -221,7 +204,7 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep,
   ep.a_policy = g_l2_hints ? 1ull : 0ull;
   ep.opt = g_epi_opt;
   if (g_nsplit == 3) return launch_one<BN, A_MN, B_MN, Producer, 3>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
-  if (g_nsplit == 2 && g_persistent) return launch_one<BN, A_MN, B_MN, Producer, 2>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
+  if (g_nsplit == 2) return launch_one<BN, A_MN, B_MN, Producer, 2>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
   return launch_one<BN, A_MN, B_MN, Producer, 1>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
 }
 void set_nsplit(int n) { g_nsplit = (n == 3) ? 3 : (n == 2 ? 2 : 1); }
@@ -231,8 +214,8 @@ static void plan_splitk(Epilogue& ep, int M, int N, int BN, int num_kb, int allo
   // N = real width of the output rows (what a split-K run has to zero); N_grid = width of the tile grid when it differs (padded wgrad taps)
   long long tiles = (long long)cdiv(M, BM) * cdiv(N_grid ? N_grid : N, BN);
   splits = 1;
-  if (allow && tiles < 148 && num_kb >= 32) {
-    splits = (int)((296 + tiles - 1) / tiles);
+  if (allow && tiles < sm_count() && num_kb >= 32) {
+    splits = (int)((2 * sm_count() + tiles - 1) / tiles);
     int maxs = num_kb / 4;      // >= 4 k-blocks (128 reduction rows) per slice: these GEMMs are latency bound, so many short slices win
     if (splits > maxs) splits = maxs;
     if (splits > 128) splits = 128;
@@ -255,12 +238,10 @@ int gemm_tf32(const float* a, long long lda, int a_mn, const float* b, long long
   if (M <= 0 || N <= 0) return 0;
   CUtensorMap ta, tb;
   int BN = (N > 64) ? 128 : 64;
-  // 128 x 256 tiles (full 512 TMEM columns with double buffering) when N allows: each A tile is fetched once per 256 columns
-  if (g_persistent && g_wide_tiles && N % 256 == 0 && (long long)cdiv(M, BM) * (N / 256) >= 120) BN = 256;
   // Latency-bound GEMMs of the token decoder (a few dozen 128-row tiles, K <= 512): when 128-wide tiles would occupy at most half of the SMs,
   // 64-wide tiles put twice as many CTAs to work -- each splits / multiplies half the B tile and drains half the accumulator, which is what a
   // single-tile-per-CTA dependent chain (TMA -> split -> MMA -> epilogue) is made of.
-  if (BN == 128 && g_persistent && g_narrow_small && (long long)cdiv(M, BM) * cdiv(N, 128) <= 74) BN = 64;
+  if (BN == 128 && g_persistent && g_narrow_small && (long long)cdiv(M, BM) * cdiv(N, 128) <= sm_count() / 2) BN = 64;
   // MN-major operands with a multiple of 32 columns: ONE grouped box per k-block instead of BM / 32 (BN / 32) four-KB boxes (rih_set_tma_grouped)
   const int a_grp = (a_mn && (g_tma_grouped & 1) && M % 32 == 0) ? 1 : 0, b_grp = (b_mn && (g_tma_grouped & 1) && N % 32 == 0) ? 1 : 0;
   if (a_mn ? (a_grp ? make_tmap_2d_grouped(&ta, a, K, M, lda, BM / 32) : make_tmap_2d(&ta, a, K, M, lda, 32, true)) : make_tmap_2d(&ta, a, M, K, lda, BM)) return 1;
@@ -272,7 +253,6 @@ int gemm_tf32(const float* a, long long lda, int a_mn, const float* b, long long
     DenseProducer<bn, am != 0, bm != 0> prod{0, 0ull, a_grp, b_grp};                                             \
     return launch_cfg<bn, am != 0, bm != 0>(ta, tb, ep, prod, M, N, num_kb, splits, kps, s); \
   }
-  RIH_TC_CASE(256, 0, 0) RIH_TC_CASE(256, 0, 1) RIH_TC_CASE(256, 1, 1)
   RIH_TC_CASE(128, 0, 0) RIH_TC_CASE(64, 0, 0)
   RIH_TC_CASE(128, 0, 1) RIH_TC_CASE(64, 0, 1)
   RIH_TC_CASE(128, 1, 1) RIH_TC_CASE(64, 1, 1)
@@ -300,7 +280,7 @@ static int make_tmap_batched(CUtensorMap* map, const BOperand& o, int B, int H, 
   CUresult r = CUDA_SUCCESS;
   for (int attempt = 0; attempt < 2; ++attempt) {
     r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(o.p), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_ERROR_INVALID_CONTEXT) break;
     cudaFree(0);
   }
@@ -342,7 +322,7 @@ void set_s2_direct(int on) { g_s2_direct = on ? 1 : 0; }
 int s2_direct() { return g_s2_direct; }
 static bool pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
-// Can the stride-1 convolution run on the tcgen05 implicit-GEMM path?
+// Can the convolution run on the tensor-core implicit-GEMM path?
 // stride 2 is supported for even H, W through a parity-stacked copy of the input (fwd, wgrad) and a zero-inserted copy of
 // dY (dgrad); both need caller-provided workspace (conv_tc_workspace).
 bool conv_tc_supported(const ConvGeom& g, int which /*0 fwd, 1 dgrad, 2 wgrad*/) {
@@ -370,7 +350,6 @@ extern "C" int rih_dilate2x(const float* y, int ldy, float* yd, int N, int Ho, i
 int conv_fwd_tf32(const float* x, const float* w, Epilogue ep, const ConvGeom& g, float* ws, cudaStream_t s) {
   const int M = g.N * g.Ho * g.Wo;
   int BN = (g.Cout > 64) ? 128 : 64;
-  if (g_persistent && g_wide_tiles && g.Cout % 256 == 0 && (long long)(M / BM) * (g.Cout / 256) >= 120) BN = 256;
   const int tile_h = (BM / g.Wo) < g.Ho ? (BM / g.Wo) : g.Ho;
   const int tile_n = BM / (g.Wo * tile_h);
   CUtensorMap ta, tb;
@@ -386,7 +365,6 @@ int conv_fwd_tf32(const float* x, const float* w, Epilogue ep, const ConvGeom& g
   if (make_tmap_2d(&tb, w, g.Cout, (long long)g.R * g.S * g.Cin, (long long)g.R * g.S * g.Cin, BN)) return 1;
   ConvTcGeom cg{g.Cin, g.Cout, g.R, g.S, g.pad, g.H, g.W, g.Ho, g.Wo, tile_h, g.stride == 2 ? (g_s2_direct ? -1 : g.N) : 0, g.Cin};
   const int num_kb = g.R * g.S * cdiv(g.Cin, BK);
-  if (BN == 256) { ConvFwdProducer<256> p{cg, 0ull}; return launch_cfg<256, false, false>(ta, tb, ep, p, M, g.Cout, num_kb, 1, num_kb, s); }
   if (BN == 128) { ConvFwdProducer<128> p{cg, 0ull}; return launch_cfg<128, false, false>(ta, tb, ep, p, M, g.Cout, num_kb, 1, num_kb, s); }
   ConvFwdProducer<64> p{cg, 0ull};
   return launch_cfg<64, false, false>(ta, tb, ep, p, M, g.Cout, num_kb, 1, num_kb, s);
@@ -398,7 +376,6 @@ static int conv_dgrad_s2_direct(const float* dy, const float* w, Epilogue ep, co
   const int H2 = g.Ho, W2 = g.Wo;                       // class grid == output grid (even H, W)
   const int M = g.N * H2 * W2;
   int BN = (g.Cin > 64) ? 128 : 64;
-  if (g_persistent && g_wide_tiles && g.Cin % 256 == 0 && (long long)(M / BM) * (g.Cin / 256) >= 120) BN = 256;
   const int tile_h = (BM / W2) < H2 ? (BM / W2) : H2;
   const int tile_n = BM / (W2 * tile_h);
   CUtensorMap ta, tb, tcm;
@@ -412,9 +389,9 @@ static int conv_dgrad_s2_direct(const float* dy, const float* w, Epilogue ep, co
   if (accumulate) { set_error("conv_dgrad_s2_direct: accumulation through an element-strided map is not supported (use the copy-based path)"); return 1; }
   bool zeroed = false;
   for (int ph = 0; ph < 2; ++ph) for (int pw = 0; pw < 2; ++pw) {
-    int rs[2], nr = 0, ss[2], ns = 0;
-    for (int r = 0; r < g.R; ++r) if (((ph + g.pad - r) & 1) == 0) rs[nr++] = r;
-    for (int q = 0; q < g.S; ++q) if (((pw + g.pad - q) & 1) == 0) ss[ns++] = q;
+    int nr = 0, ns = 0;
+    for (int r = 0; r < g.R; ++r) if (((ph + g.pad - r) & 1) == 0) ++nr;
+    for (int q = 0; q < g.S; ++q) if (((pw + g.pad - q) & 1) == 0) ++ns;
     if (nr * ns == 0) {
       if (!accumulate && !zeroed) {      // this class receives no gradient: zero the whole tensor once, the other classes overwrite their pixels
         if (ep.ldc == g.Cin) cudaMemsetAsync(ep.c, 0, (size_t)g.N * g.H * g.W * g.Cin * sizeof(float), s);
@@ -440,7 +417,7 @@ static int conv_dgrad_s2_direct(const float* dy, const float* w, Epilogue ep, co
 #define RIH_S2_CASE(bn)                                                                                                        \
     { ConvDgradS2Producer<bn> p{cg, nt, {tap[0], tap[1], tap[2], tap[3]}, {dr[0], dr[1], dr[2], dr[3]}, {ds[0], ds[1], ds[2], ds[3]}, b_grp}; \
       rc = launch_cfg<bn, false, true>(ta, tb, e2, p, M, g.Cin, num_kb, 1, num_kb, s, &tcm); }
-    if (BN == 256) RIH_S2_CASE(256) else if (BN == 128) RIH_S2_CASE(128) else RIH_S2_CASE(64)
+    if (BN == 128) RIH_S2_CASE(128) else RIH_S2_CASE(64)
 #undef RIH_S2_CASE
     if (rc) return rc;
   }
@@ -457,7 +434,6 @@ int conv_dgrad_tf32(const float* dy, const float* w, Epilogue ep, const ConvGeom
   }
   const int M = g.N * g.H * g.W;
   int BN = (g.Cin > 64) ? 128 : 64;
-  if (g_persistent && g_wide_tiles && g.Cin % 256 == 0 && (long long)(M / BM) * (g.Cin / 256) >= 120) BN = 256;
   const int tile_h = (BM / g.W) < g.H ? (BM / g.W) : g.H;
   const int tile_n = BM / (g.W * tile_h);
   CUtensorMap ta, tb;
@@ -468,7 +444,6 @@ int conv_dgrad_tf32(const float* dy, const float* w, Epilogue ep, const ConvGeom
             : make_tmap_2d(&tb, w, g.Cout, (long long)g.R * g.S * g.Cin, (long long)g.R * g.S * g.Cin, 32, true)) return 1;
   ConvTcGeom cg{g.Cin, g.Cout, g.R, g.S, g.pad, g.H, g.W, g.Ho, g.Wo, tile_h, 0, g.Cin};
   const int num_kb = g.R * g.S * cdiv(g.Cout, BK);
-  if (BN == 256) { ConvDgradProducer<256> p{cg, b_grp}; return launch_cfg<256, false, true>(ta, tb, ep, p, M, g.Cin, num_kb, 1, num_kb, s); }
   if (BN == 128) { ConvDgradProducer<128> p{cg, b_grp}; return launch_cfg<128, false, true>(ta, tb, ep, p, M, g.Cin, num_kb, 1, num_kb, s); }
   ConvDgradProducer<64> p{cg, b_grp};
   return launch_cfg<64, false, true>(ta, tb, ep, p, M, g.Cin, num_kb, 1, num_kb, s);
@@ -492,22 +467,22 @@ int stem_wgrad_tf32(const float* dy, int lddy, const float* xp, Epilogue ep, int
   if (make_tmap_2d(&ta, dy, P, 64, lddy, 32, true)) return 1;
   if (make_tmap_stem(&tb, xp, N, H + 6, W + 8, Wo, 32, true)) return 1;
   int num_kb = P / BK, splits, kps;
-  plan_splitk(ep, 64, 224, 256, num_kb, 1, splits, kps, s);
-  StemWgradProducer<256> p{Ho, Wo};
-  return launch_cfg<256, true, true>(ta, tb, ep, p, 64, 224, num_kb, splits, kps, s);
+  plan_splitk(ep, 64, 224, 128, num_kb, 1, splits, kps, s);
+  StemWgradProducer<128> p{Ho, Wo};
+  return launch_cfg<128, true, true>(ta, tb, ep, p, 64, 224, num_kb, splits, kps, s);
 }
 
 int conv_wgrad_tf32(const float* dy, const float* x, Epilogue ep, const ConvGeom& g, float* ws, cudaStream_t s) {
   const int P = g.N * g.Ho * g.Wo, taps = g.R * g.S, Nn = taps * g.Cin;
-  // Cin a multiple of 32: the 32-column chunks of an N tile never straddle a tap, so 256-wide tiles may span several taps (the dY operand is
-  // re-read once per N tile: 3 times instead of 9 for Cin = 64, 9 instead of 18 for Cin = 256) -- RIH_WGRAD_WIDE=0 keeps one tap per tile
+  // Cin a multiple of 32: the 32-column chunks of an N tile never straddle a tap, so 128-wide tiles may span several taps (Cin = 32, 64:
+  // the dY operand is re-read once per N tile instead of once per tap and channel block) -- RIH_WGRAD_WIDE=0 keeps one tap per tile
   // Channel counts that are not multiples of 32 (HRNet's 48, 80, 208 ...) take the wide tiles too, on a "virtual" grid of cin32 = ceil32(Cin)
-  // columns per tap (rih_set_wgrad_wide bit 1): 48-channel convolutions ran nine 64-wide tiles (dY re-read 9 times, 240 us vs 53 us for the
-  // 96-channel convolutions of equal flops in the HRNet-w48 step); three 256-wide tiles over 9 x 64 virtual columns instead.
+  // columns per tap (rih_set_wgrad_wide bit 1): 48-channel convolutions would otherwise run nine 64-wide tiles (dY re-read 9 times);
+  // five 128-wide tiles over 9 x 64 virtual columns instead.
   const int cin32 = cdiv(g.Cin, 32) * 32;
-  const bool wide_pad = (g_wgrad_wide & 2) && g.Cin % 32 != 0 && g.Cin % 4 == 0 && taps * cin32 >= 256;
-  const bool wide = g_wgrad_wide && g_persistent && (g.Cin % 32 == 0 || wide_pad) && Nn >= 256;
-  const int BN = wide ? 256 : ((g.Cin % 128 == 0) ? 128 : 64);
+  const bool wide_pad = (g_wgrad_wide & 2) && g.Cin % 32 != 0 && g.Cin % 4 == 0 && taps * cin32 >= 128;
+  const bool wide = g_wgrad_wide && g_persistent && (g.Cin % 32 == 0 || wide_pad) && Nn >= 128;
+  const int BN = wide ? 128 : ((g.Cin % 128 == 0) ? 128 : 64);
   // N tiles never straddle a tap: each tap owns ceil(Cin / BN) tiles; when BN does not divide Cin (48, 96, ...) the tile grid is
   // "virtual" (cin_pad columns per tap) and the epilogue stores through a 3-D map [Cout][taps][Cin] that clips at the tap's edge
   const int cin_pad = wide ? cin32 : cdiv(g.Cin, BN) * BN, Ngrid = taps * cin_pad;
@@ -515,11 +490,11 @@ int conv_wgrad_tf32(const float* dy, const float* x, Epilogue ep, const ConvGeom
   CUtensorMap ta, tb, tcm;
   const int a_grp = ((g_tma_grouped & 1) && g.Cout % 32 == 0) ? 1 : 0;
   if (a_grp ? make_tmap_2d_grouped(&ta, dy, P, g.Cout, g.ldy, BM / 32) : make_tmap_2d(&ta, dy, P, g.Cout, g.ldy, 32, true)) return 1;
-  // input chunks of one tap merged into grouped rank-5 boxes (rih_set_tma_grouped bit 1): b_grp = gcd(chunks per tap, 8) consecutive chunks per box
+  // input chunks of one tap merged into grouped rank-5 boxes (rih_set_tma_grouped bit 1): b_grp = gcd(chunks per tap, 4) consecutive chunks per box
   int b_grp = 0;
   if ((g_tma_grouped & 2) && wide && !wide_pad && (g.stride == 1 || g_s2_direct)) {
     const int per_tap = g.Cin / 32;
-    b_grp = (per_tap % 8 == 0) ? 8 : ((per_tap % 4 == 0) ? 4 : ((per_tap % 2 == 0) ? 2 : 0));
+    b_grp = (per_tap % 4 == 0) ? 4 : ((per_tap % 2 == 0) ? 2 : 0);
   }
   if (b_grp) {
     if (make_tmap_nhwc_grouped(&tb, x, g.N, g.H, g.W, g.Cin, g.ldx, bw, bh, g.stride == 2 ? 2 : 1, b_grp)) return 1;
@@ -541,8 +516,7 @@ int conv_wgrad_tf32(const float* dy, const float* x, Epilogue ep, const ConvGeom
     if (make_tmap_wgrad_out(&tcm, ep.c, g.Cout, taps, g.Cin)) return 1;
     cmap = &tcm; ep.nv_pad = cin_pad; ep.nv_real = g.Cin;
   }
-  if (BN == 256) { ConvWgradProducer<256> p{cg, a_grp, b_grp}; return launch_cfg<256, true, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap); }
-  if (BN == 128) { ConvWgradProducer<128> p{cg, a_grp, 0}; return launch_cfg<128, true, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap); }
+  if (BN == 128) { ConvWgradProducer<128> p{cg, a_grp, wide ? b_grp : 0}; return launch_cfg<128, true, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap); }
   ConvWgradProducer<64> p{cg, a_grp, 0};
   return launch_cfg<64, true, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap);
 }
@@ -552,18 +526,17 @@ int conv_wgrad_tf32(const float* dy, const float* x, Epilogue ep, const ConvGeom
 
 using namespace rih;
 
-// Raw tcgen05 GEMM entry point (testing / benchmarking of the tensor-core path in isolation):
+// Raw tensor-core GEMM entry point (testing / benchmarking of the tensor-core path in isolation):
 //   c[M,N] (+)= op(a) * op(b)^T ; a_mn/b_mn select MN-major ([K,M] / [K,N] row-major) operands.
 RIH_API int rih_gemm_tf32(const float* a, long long lda, int a_mn, const float* b, long long ldb, int b_mn, float* c, int ldc,
                           int M, int N, int K, const float* bias, int relu, int accumulate, int allow_splitk, int nsplit, cudaStream_t stream) {
   RIH_REQUIRE(M >= 0 && N > 0 && K > 0, "gemm_tf32: bad shape");
-  // nsplit: 1 = TF32, 3 = 3xTF32.  Debug variants: negative = per-thread-store epilogue, +10 = non-persistent kernel.
+  // nsplit: 1 = TF32, 3 = 3xTF32.  Debug variants: negative = per-thread-store epilogue, +10 = non-persistent kernel, +20 = narrow tiles
+  // (accepted for compatibility: the tiles are at most 128 wide on every path).
   int v = nsplit < 0 ? -nsplit : nsplit;
-  const int narrow = v >= 20;
-  if (narrow) v -= 20;
+  if (v >= 20) v -= 20;
   const int nonpersistent = v >= 10;
   if (nonpersistent) v -= 10;
-  tc::set_wide_tiles(!narrow);
   RIH_REQUIRE(v == 1 || v == 2 || v == 3, "gemm_tf32: nsplit must be 1 (TF32, truncating), 2 (TF32, round-to-nearest) or 3 (3xTF32)");
   tc::set_tma_epilogue(nsplit > 0);
   tc::set_persistent(!nonpersistent);
@@ -573,6 +546,5 @@ RIH_API int rih_gemm_tf32(const float* a, long long lda, int a_mn, const float* 
   int rc = tc::gemm_tf32(a, lda, a_mn, b, ldb, b_mn, ep, M, N, K, allow_splitk, stream);
   tc::set_tma_epilogue(1);
   tc::set_persistent(1);
-  tc::set_wide_tiles(1);
   return rc;
 }

@@ -1,10 +1,11 @@
-// tcgen05 (5th-gen tensor core) TF32 GEMM for sm_100a: TMA -> 128B-swizzled shared memory -> tcgen05.mma with the
-// fp32 accumulator in TMEM -> tcgen05.ld epilogue.  Hand-written PTX, no CUTLASS.
+// Hopper (sm_90a) TF32 GEMM: TMA -> 128B-swizzled shared memory -> wgmma.mma_async with the fp32 accumulator in registers of the
+// consumer warpgroups -> shared-memory staging -> TMA-store epilogue.  Hand-written PTX, no CUTLASS.
 //   D[M,N] (+)= A(M x K) * B(N x K)^T,  fp32 storage, TF32 multiplicands, fp32 accumulation.
 // Operand tiles are [rows x 128 bytes] TMA boxes with SWIZZLE_128B; the same box format serves
 //   K-major  operands (rows = M/N index, 32 consecutive k per row)          and
 //   MN-major operands (rows = k index, 32 consecutive m/n per row; one box per 32-wide m/n chunk).
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer, warps 2..5 = epilogue.
+// wgmma reads TF32 operands K-major only, so MN-major tiles are transposed in shared memory by a preparation warpgroup (which also
+// rounds / splits the operands of the TF32-rn and 3xTF32 kernels) before the consumers multiply them.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -13,10 +14,9 @@
 namespace rih {
 namespace tc {
 
-constexpr int BM = 128;          // UMMA M
+constexpr int BM = 128;          // two consumer warpgroups x wgmma M = 64
 constexpr int BK = 32;           // fp32 elements per stage row = 128 bytes = one swizzle span
-constexpr int UMMA_K = 8;        // tf32: 32 bytes per instruction
-constexpr int THREADS = 192;
+constexpr int WG_K = 8;          // tf32: 32 bytes per wgmma instruction
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -43,8 +43,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
   asm volatile(
@@ -65,7 +63,7 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* map, i
       : "memory");
 }
 // L2 eviction-priority hints for streamed operands: an activation tile a GEMM reads once should not push the output of the previous
-// kernel (which the next kernel is about to read) out of the 126 MB L2.
+// kernel (which the next kernel is about to read) out of the 50 MB L2.
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -124,89 +122,53 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-// tcgen05 shared-memory matrix descriptor (PTX ISA "matrix descriptor", sm_100 version bit set), SWIZZLE_128B.
-//   bits [0,14)  start address >> 4      bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4 bits [46,48) version = 1     bits [61,64) layout type (2 = SWIZZLE_128B)
-//   layout type 1 = SWIZZLE_128B_BASE32B (32-byte swizzle atoms: the only layout tcgen05 accepts for MN-major TF32 operands)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout = 2) {
+// wgmma shared-memory matrix descriptor (sm_90), K-major SWIZZLE_128B: 8-row groups of 128-byte rows are 1024 B apart (stride byte
+// offset); the leading byte offset is unused for swizzled K-major layouts.  A K step of 8 tf32 advances the start address by 32 B.
+__device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout << 61;
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;          // layout type 1 = SWIZZLE_128B
   return d;
 }
-// instruction descriptor for kind::tf32, fp32 accumulate, M = 128
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int n, bool a_mn, bool b_mn) {
-  return (1u << 4)            // D format F32
-       | (2u << 7)            // A format TF32
-       | (2u << 10)           // B format TF32
-       | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16)
-       | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// d[64 x BN] += A(64 x 8, K-major smem) * B(BN x 8, K-major smem)^T; per thread BN / 2 fp32 accumulators in the wgmma D fragment layout
+template <int BN> __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc);
+template <> __device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
+template <> __device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc) : "memory");
 }
 
-// NSPLIT = 1: single-pass TF32 (hardware truncates the fp32 operands).  NSPLIT = 2: single-pass TF32 with the operands
-// rounded to nearest in shared memory first (unbiased, what cuDNN/cuBLAS TF32 do).  NSPLIT = 3: error-compensated "3xTF32": every operand tile is split in shared memory into
-// hi = value rounded to TF32 and lo = value - hi (exact in fp32), and D += hi*hi + lo*hi + hi*lo  (fp32-faithful).
+// NSPLIT = 1: single-pass TF32 (the tensor core ignores the low mantissa bits of the fp32 operands).  NSPLIT = 2: single-pass TF32 with the
+// operands rounded to nearest in shared memory first (unbiased, what cuDNN/cuBLAS TF32 do).  NSPLIT = 3: error-compensated "3xTF32": every
+// operand tile is split in shared memory into hi = value rounded to TF32 and lo = value - hi (exact in fp32), and D += hi*hi + lo*hi + hi*lo
+// (fp32-faithful).
 template <int BN, int NSPLIT> __host__ __device__ constexpr int stage_bytes() { return (BM * 128 + BN * 128) * (NSPLIT == 3 ? 2 : 1); }
-// Build-time tuning knobs (A/B variants of the library are built by renderih_b200/_build.build_variant):
-//   RIH_EPI_WGS   epilogue warpgroups of the single-pass TF32 persistent kernels (default 2)
-//   RIH_DEEP      1 = as many shared-memory stages as fit next to the staging tiles for the single-pass TF32 kernels
-#ifndef RIH_EPI_WGS
-#define RIH_EPI_WGS 2
-#endif
-#ifndef RIH_DEEP
-#define RIH_DEEP 1      // measured on the ResNet-50 trunk (tools/trunk_bench.py): 20.85 -> 20.53 ms fwd+bwd
-#endif
+// accumulator staging: the consumers park the 128 x BN tile as BN / 32 SWIZZLE_128B [128 rows x 128 B] chunks, each the source of one TMA store
+template <int BN> __host__ __device__ constexpr int acc_bytes() { return BM * BN * 4; }
+// as many stages as fit next to the accumulator staging in the 227 KB an H100 CTA may use (at most 8)
 template <int BN, int NSPLIT> __host__ __device__ constexpr int num_stages() {
-  if (NSPLIT == 1 && RIH_DEEP) {
-    // 227 KB per CTA - staging (32 KB per epilogue warpgroup) - barriers, in units of one stage (24 / 32 / 48 KB for BN = 64 / 128 / 256)
-    return (227 * 1024 - 32 * 1024 * RIH_EPI_WGS - 2048) / ((BM + BN) * 128);
-  }
-  return (BN >= 256 && NSPLIT == 3) ? 2 : (BN >= 128 ? 3 : 4);
+  return (227 * 1024 - acc_bytes<BN>() - 3 * 1024) / stage_bytes<BN, NSPLIT>() > 8 ? 8 : (227 * 1024 - acc_bytes<BN>() - 3 * 1024) / stage_bytes<BN, NSPLIT>();
 }
-constexpr int EPI_STAGING_BYTES = 2 * BM * 128;   // two [128 x 32 fp32] staging tiles for the TMA-store epilogue (per epilogue warpgroup)
-// Epilogue warpgroups of the persistent kernel.  The single-pass TF32 kernels (NSPLIT = 1) have no splitter warps and room in shared memory, so
-// they run TWO epilogue warpgroups that take alternate 32-column chunks of the accumulator (each with its own pair of staging tiles, its own
-// named barrier and its own TMA-store bulk groups): the store-bound 1x1 convolutions (K = 64 ... 256, 128 KB of output per 128 x 256 tile)
-// were limited by the serial tcgen05.ld -> st.shared -> barrier -> TMA-store chain of one warpgroup (3.6 TB/s of 6.5).
-template <int NSPLIT> __host__ __device__ constexpr int epi_wgs() { return NSPLIT == 1 ? RIH_EPI_WGS : 1; }
-template <int BN, int NSPLIT> __host__ __device__ constexpr int smem_base_bytes() {
-  return num_stages<BN, NSPLIT>() * stage_bytes<BN, NSPLIT>() + EPI_STAGING_BYTES * epi_wgs<NSPLIT>() + 1024 + 256;
+// Per-column epilogue vectors of the tile's BN columns cached in shared memory: [0] = multiplicative (folded BatchNorm scale), [1] = additive
+// (bias or folded BatchNorm shift).  Every epilogue thread needs all 32 values of a chunk: 16 broadcast LDS.128 instead of 64 broadcast LDG.32.
+template <int BN> __host__ __device__ constexpr int colvec_bytes() { return 2 * BN * 4; }
+template <int BN, int NSPLIT> __host__ __device__ constexpr int smem_bytes() {
+  return num_stages<BN, NSPLIT>() * stage_bytes<BN, NSPLIT>() + acc_bytes<BN>() + 256 + colvec_bytes<BN>() + 1024;
 }
-// Per-column epilogue vectors of the tile's BN columns cached in shared memory (persistent kernel): [0] = multiplicative (folded BatchNorm scale),
-// [1] = additive (bias or folded BatchNorm shift).  Every epilogue thread needs all 32 values of a chunk: 16 broadcast LDS.128 instead of 64
-// broadcast LDG.32 per chunk.  Only when it fits next to the stage ring (it does not for 3xTF32 128 x 256 tiles: global loads there).
-template <int BN, int NSPLIT> __host__ __device__ constexpr int colvec_bytes() {
-  return (smem_base_bytes<BN, NSPLIT>() + 2 * BN * 4 <= 227 * 1024) ? 2 * BN * 4 : 0;
-}
-template <int BN, int NSPLIT> __host__ __device__ constexpr int smem_bytes() { return smem_base_bytes<BN, NSPLIT>() + colvec_bytes<BN, NSPLIT>(); }
 
 // ---------------------------------------------------------------- producers (TMA issue logic, one elected lane)
 // Each producer loads, for k-block `kb`, the A tile (BM x 32) to `sa` and the B tile (BN x 32) to `sb`.
@@ -550,202 +512,90 @@ __device__ __forceinline__ void load_res_chunk(float4 (&r)[8], const Epilogue& e
 }
 
 
-// ---------------------------------------------------------------- the kernel
-// tma_epi != 0: the epilogue stages 32-column chunks in 128B-swizzled shared memory and writes them with TMA stores
-// (cp.reduce.async.bulk ... .add for accumulate / split-K), fully coalesced and clipped at the tensor edge by the hardware.
-template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT>
-__global__ void __launch_bounds__(THREADS)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_c,
-               Epilogue ep, Producer prod, int num_kb_total, int kb_per_split, int tma_epi) {
-  constexpr int STAGES = num_stages<BN, NSPLIT>();
-  constexpr int A_BYTES = BM * 128, B_BYTES = BN * 128, AB_BYTES = A_BYTES + B_BYTES;
-  constexpr int STAGE_BYTES = stage_bytes<BN, NSPLIT>();   // [A | B] (+ [A_lo | B_lo] when NSPLIT == 3)
-  constexpr uint32_t IDESC = make_idesc_tf32(BN, A_MN, B_MN);
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* staging = smem + STAGES * STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + EPI_STAGING_BYTES);
-  uint64_t* full = bars;                 // [STAGES] TMA bytes landed
-  uint64_t* empty = bars + STAGES;       // [STAGES] MMAs finished reading the stage
-  uint64_t* ready = bars + 2 * STAGES;   // [STAGES] hi/lo split written (NSPLIT == 3 only)
-  uint64_t* tmem_full = bars + 3 * STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * STAGES + 1);
-
-  pdl_launch_dependents();     // the stream successor may start its own prologue now; it blocks in its pdl_wait() until this grid is done
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-  const int kb_beg = blockIdx.z * kb_per_split;
-  const int num_kb = min(num_kb_total - kb_beg, kb_per_split);
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    if (tma_epi) tma_prefetch_desc(&tmap_c);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); mbar_init(&ready[s], 128); }
-    mbar_init(tmem_full, 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)BN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();                  // prologue done (barriers, TMEM, descriptors): from here on the kernel reads what its stream predecessor wrote
-
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(&empty[s], ph ^ 1);
-        mbar_expect_tx(&full[s], AB_BYTES);
-        uint8_t* sa = smem + s * STAGE_BYTES;
-        prod.template load<false>(&tmap_a, &tmap_b, kb_beg + kb, m0, n0, 0, sa, sa + A_BYTES, &full[s], 0);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(NSPLIT == 3 ? &ready[s] : &full[s], ph);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
-        const uint32_t sb = sa + A_BYTES;
+// ---------------------------------------------------------------- operand preparation (transpose / round / split in shared memory)
+__device__ __forceinline__ void prep_bar_sync() { asm volatile("bar.sync 3, 128;" ::: "memory"); }
+__device__ __forceinline__ void cons_bar_sync() { asm volatile("bar.sync 4, 256;" ::: "memory"); }
+template <int NSPLIT> __device__ __forceinline__ void split_tf32(float4 v, float4& h, float4& l) {
+  if constexpr (NSPLIT == 1) { h = v; return; }
+  // hi = round-to-nearest TF32 (10-bit mantissa): unbiased, so the dropped lo*lo term and the tensor core's truncation of lo do not
+  // accumulate coherently over K
+  h.x = __uint_as_float((__float_as_uint(v.x) + 0x1000u) & 0xFFFFE000u);
+  h.y = __uint_as_float((__float_as_uint(v.y) + 0x1000u) & 0xFFFFE000u);
+  h.z = __uint_as_float((__float_as_uint(v.z) + 0x1000u) & 0xFFFFE000u);
+  h.w = __uint_as_float((__float_as_uint(v.w) + 0x1000u) & 0xFFFFE000u);
+  l = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
+}
+// One operand tile of R rows (m or n) by BK k.  MN-major: the TMA delivered R / 32 chunks of [32 k rows x 128 B]; they are rewritten in place
+// as the K-major [R rows x 128 B] tile wgmma reads (both SWIZZLE_128B: 16-byte unit j of row r sits at unit j ^ (r & 7)).  Every one of the
+// 128 preparation threads gathers its units into registers before any thread writes.  lo != nullptr: NSPLIT == 3 low parts.
+template <int R, bool MN, int NSPLIT>
+__device__ __forceinline__ void prep_operand(uint8_t* hi, uint8_t* lo, int p) {
+  if constexpr (MN) {
+    constexpr int U = R * 8 / 128;
+    float4 g[U];
 #pragma unroll
-        for (int k = 0; k < BK / UMMA_K; ++k) {
-          // K-major (SWIZZLE_128B): 8-row groups are 1024 B apart (SBO), a K step of 8 tf32 = +32 B inside the swizzle span.
-          // MN-major (SWIZZLE_128B_BASE32B, TMA 128B_ATOM_32B): 32-wide m/n chunks are BK*128 B apart (LBO), 4-row k groups
-          // are 512 B apart (SBO), a K step of 8 rows = +1024 B.
-          uint64_t ad = A_MN ? make_smem_desc(sa + k * 1024, BK * 128, 512, 1) : make_smem_desc(sa + k * 32, 16, 1024, 2);
-          uint64_t bd = B_MN ? make_smem_desc(sb + k * 1024, BK * 128, 512, 1) : make_smem_desc(sb + k * 32, 16, 1024, 2);
-          umma_tf32(tmem_base, ad, bd, IDESC, (kb | k) ? 1u : 0u);
-          if constexpr (NSPLIT == 3) {
-            // descriptors address in 16-byte units: the lo copies sit AB_BYTES after the hi tiles
-            const uint64_t lo_off = (uint64_t)(AB_BYTES >> 4);
-            umma_tf32(tmem_base, ad + lo_off, bd, IDESC, 1u);   // lo(A) * hi(B)
-            umma_tf32(tmem_base, ad, bd + lo_off, IDESC, 1u);   // hi(A) * lo(B)
-          }
-        }
-        umma_commit(&empty[s]);
+    for (int i = 0; i < U; ++i) {
+      const int u = p + i * 128, m = u % R, kq = u / R;
+      const uint8_t* src = hi + (m >> 5) * (BK * 128);
+      const int mm = m & 31;
+      float x[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int k = kq * 4 + e;
+        x[e] = *reinterpret_cast<const float*>(src + k * 128 + ((((mm >> 2) ^ (k & 7)) << 4) | ((mm & 3) << 2)));
       }
-      umma_commit(tmem_full);
+      g[i] = make_float4(x[0], x[1], x[2], x[3]);
     }
-  } else {
-    // warps 2..5: (NSPLIT == 3) hi/lo splitter during the main loop, then the epilogue.
-    if constexpr (NSPLIT == 3) {
-      const int t = threadIdx.x - 64;   // 0..127
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(&full[s], ph);
-        uint4* hi = reinterpret_cast<uint4*>(smem + s * STAGE_BYTES);
-        uint4* lo = reinterpret_cast<uint4*>(smem + s * STAGE_BYTES + AB_BYTES);
+    prep_bar_sync();
+#pragma unroll
+    for (int i = 0; i < U; ++i) {
+      const int u = p + i * 128, m = u % R, kq = u / R;
+      const int off = m * 128 + ((kq ^ (m & 7)) << 4);
+      float4 h, l;
+      split_tf32<NSPLIT>(g[i], h, l);
+      *reinterpret_cast<float4*>(hi + off) = h;
+      if constexpr (NSPLIT == 3) *reinterpret_cast<float4*>(lo + off) = l;
+    }
+  } else if constexpr (NSPLIT >= 2) {
 #pragma unroll 4
-        for (int i = t; i < AB_BYTES / 16; i += 128) {
-          uint4 v = hi[i];
-          // hi = round-to-nearest TF32 (10-bit mantissa): unbiased, so the dropped lo*lo term and the hardware's truncation of lo
-          // do not accumulate coherently over K
-          uint4 h = make_uint4((v.x + 0x1000u) & 0xFFFFE000u, (v.y + 0x1000u) & 0xFFFFE000u, (v.z + 0x1000u) & 0xFFFFE000u, (v.w + 0x1000u) & 0xFFFFE000u);
-          uint4 l;
-          l.x = __float_as_uint(__uint_as_float(v.x) - __uint_as_float(h.x));
-          l.y = __float_as_uint(__uint_as_float(v.y) - __uint_as_float(h.y));
-          l.z = __float_as_uint(__uint_as_float(v.z) - __uint_as_float(h.z));
-          l.w = __float_as_uint(__uint_as_float(v.w) - __uint_as_float(h.w));
-          hi[i] = h;
-          lo[i] = l;
-        }
-        fence_proxy_async();     // generic-proxy smem writes -> visible to the tensor core (async proxy)
-        mbar_arrive(&ready[s]);
-      }
+    for (int i = p; i < R * 8; i += 128) {
+      float4 h, l;
+      split_tf32<NSPLIT>(reinterpret_cast<float4*>(hi)[i], h, l);
+      reinterpret_cast<float4*>(hi)[i] = h;
+      if constexpr (NSPLIT == 3) reinterpret_cast<float4*>(lo)[i] = l;
     }
-    // TMEM lane quarters (warp % 4)
-    const int q = warp & 3;
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    const int rr = q * 32 + lane;       // row inside the tile
-    const int m = m0 + rr;
-    if (num_kb > 0 && tma_epi) {
-      const bool elected = (threadIdx.x == 64);
-      const unsigned long long dseed = ep.thresh ? (*ep.seed_ptr + ep.site * 0xD1B54A32D192ED03ull) : 0ull;
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-        const int nb = n0 + c * 32;
-        epilogue_math(v, ep, m, nb, dseed);
-        if (c >= 2) {                    // staging buffer (c & 1) must have been read out by its previous TMA store
-          if (elected) tma_store_wait_read<1>();
-          epi_bar_sync();
-        }
-        uint8_t* buf = staging + (c & 1) * (BM * 128);
-#pragma unroll
-        for (int j = 0; j < 8; ++j)      // 16-byte chunk j of row rr lives at chunk (j ^ (rr & 7)): the SWIZZLE_128B pattern
-          *reinterpret_cast<float4*>(buf + rr * 128 + ((j ^ (rr & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        fence_proxy_async();
-        epi_bar_sync();
-        if (elected) {
-          if (ep.mode == 0) tma_store_2d(&tmap_c, buf, nb, m0);
-          else tma_reduce_add_2d(&tmap_c, buf, nb, m0);
-          tma_store_commit();
-        }
-      }
-      if (elected) tma_store_wait<0>();
-    } else if (num_kb > 0) {
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          ep.store4(m, n0 + c * 32 + j * 4, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)BN) : "memory");
   }
 }
 
-// ---------------------------------------------------------------- persistent variant
-// One CTA per SM loops over output tiles (static round-robin).  The shared-memory stage ring runs continuously across
-// tiles, the accumulator is double-buffered in TMEM (2 x BN columns) and the epilogue has its own four warps, so the
-// TMA stores of tile i overlap the loads / MMAs of tile i+1 and the per-CTA prologue (TMEM allocation, barrier init,
-// descriptor fetch) is paid once per SM instead of once per tile.
-//   warp 0 = TMA producer | warp 1 = MMA issuer + TMEM owner | warps 2..9 = hi/lo splitter (NSPLIT >= 2 only) |
-//   last 4 warps = epilogue (TMEM -> registers -> swizzled smem -> TMA store / reduce-add)
-constexpr int SPLIT_WARPS = 8;   // hi/lo splitter warps of the persistent kernel (NSPLIT >= 2): the split pass (32-48 KB of shared memory per k-block) is what
-                                 // bounds the many small, latency-bound 3xTF32 GEMMs of the decoder -- 8 warps halve it against the original 4
-template <int NSPLIT> __host__ __device__ constexpr int persistent_threads() { return NSPLIT >= 2 ? (2 + SPLIT_WARPS + 4) * 32 : (2 + 4 * epi_wgs<NSPLIT>()) * 32; }
+// ---------------------------------------------------------------- the kernel
+// Persistent: the grid is at most one CTA per SM and loops over output tiles (static round-robin); a grid of one CTA per tile is the
+// non-persistent form.  The shared-memory stage ring runs continuously across tiles, so the TMA loads of tile i+1 overlap the epilogue of tile i.
+//   warpgroup 0: warp 0 = TMA producer (warps 1-3 idle)
+//   warpgroup 1 (only when an operand is MN-major or NSPLIT >= 2): operand preparation (prep_operand)
+//   last two warpgroups: consumers -- wgmma over rows [64 wg, 64 wg + 64) of the tile, then the epilogue of the chunks c with c % 2 == wg
+// tma_epi != 0: the epilogue writes 32-column chunks with TMA stores (cp.reduce.async.bulk ... .add for accumulate / split-K), fully coalesced
+// and clipped at the tensor edge by the hardware.
+template <bool A_MN, bool B_MN, int NSPLIT> __host__ __device__ constexpr bool has_prep() { return A_MN || B_MN || NSPLIT >= 2; }
+template <bool A_MN, bool B_MN, int NSPLIT> __host__ __device__ constexpr int persistent_threads() { return (has_prep<A_MN, B_MN, NSPLIT>() ? 4 : 3) * 128; }
 
 template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT>
-__global__ void __launch_bounds__(persistent_threads<NSPLIT>())
+__global__ void __launch_bounds__(persistent_threads<A_MN, B_MN, NSPLIT>(), 1)
 gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_c,
                           Epilogue ep, Producer prod, int num_kb_total, int kb_per_split, int tiles_m, int tiles_n, int splits, int tma_epi) {
   constexpr int STAGES = num_stages<BN, NSPLIT>();
   constexpr int A_BYTES = BM * 128, B_BYTES = BN * 128, AB_BYTES = A_BYTES + B_BYTES;
   constexpr int STAGE_BYTES = stage_bytes<BN, NSPLIT>();
-  constexpr uint32_t IDESC = make_idesc_tf32(BN, A_MN, B_MN);
-  constexpr int EPI_WARP0 = (NSPLIT >= 2) ? 2 + SPLIT_WARPS : 2;
-  constexpr int EPI_WG = epi_wgs<NSPLIT>();
-  constexpr uint32_t TMEM_COLS = 2 * BN;
+  constexpr bool PREP = has_prep<A_MN, B_MN, NSPLIT>();
+  constexpr int CONS_WARP0 = PREP ? 8 : 4;
+  constexpr int EPI_WG = 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* staging = smem + STAGES * STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + EPI_STAGING_BYTES * EPI_WG);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + STAGES;
-  uint64_t* ready = bars + 2 * STAGES;
-  uint64_t* tmem_full = bars + 3 * STAGES;       // [2]
-  uint64_t* tmem_empty = bars + 3 * STAGES + 2;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * STAGES + 4);
-  constexpr bool COLVEC = colvec_bytes<BN, NSPLIT>() > 0;
-  float* const colvec = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);      // [2][BN] when COLVEC
+  uint8_t* accbuf = smem + STAGES * STAGE_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(accbuf + acc_bytes<BN>());
+  uint64_t* full = bars;                 // [STAGES] TMA bytes landed
+  uint64_t* empty = bars + STAGES;       // [STAGES] consumers finished reading the stage
+  uint64_t* ready = bars + 2 * STAGES;   // [STAGES] operands prepared (PREP only)
+  float* const colvec = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);      // [2][BN]
 
   pdl_launch_dependents();     // the stream successor may start its own prologue now; it blocks in its pdl_wait() until this grid is done
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -755,19 +605,11 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     if (tma_epi) tma_prefetch_desc(&tmap_c);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); mbar_init(&ready[s], SPLIT_WARPS * 32); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], 128 * EPI_WG); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); mbar_init(&ready[s], 128); }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();                  // prologue done (barriers, TMEM, descriptors): from here on the kernel reads what its stream predecessor wrote
+  pdl_wait();                  // prologue done (barriers, descriptors): from here on the kernel reads what its stream predecessor wrote
 
   // third tile coordinate z: split-K slice (kb_beg = z * kb_per_split), or -- batched GEMM (ep.batch_heads != 0) -- the batch index
   const bool batched = ep.batch_heads != 0;
@@ -785,7 +627,6 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
   if (warp == 0) {
     // Producers with many small boxes per k-block (MN-major operands: the weight-gradient GEMMs) produce with the whole warp: lane 0 waits for
     // the stage and arms its barrier, then every lane issues its box (Producer::load<true>).  ep.opt bit 2 = 0 keeps the single-thread issue.
-    // (Measured: ConvWgrad kernels 3.38 -> 2.15 ms per step; producers with one or two large boxes were SLOWER warp-wide and stay single-thread.)
     const bool wide_issue = Producer::WIDE_OK && (ep.opt & 4) != 0;
     if (lane == 0 || wide_issue) {
       uint32_t it = 0;
@@ -804,8 +645,7 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
           if (wide_issue) __syncwarp();
           uint8_t* sa = smem + s * STAGE_BYTES;
           // k-block rotation: the sum over k does not care about the order, so each tile starts at its own k-block and wraps around --
-          // CTAs that run in lockstep then fetch DIFFERENT 128-byte slices of their (1 KB-pitch) rows at any instant instead of all hitting
-          // the same address bits [7, 10) of every row
+          // CTAs that run in lockstep then fetch DIFFERENT 128-byte slices of their (1 KB-pitch) rows at any instant
           int kk = kb;
           if (ep.kb_rotate) { kk = kb + (t % nkb); if (kk >= nkb) kk -= nkb; }
           if constexpr (Producer::WIDE_OK) {
@@ -817,42 +657,10 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      uint32_t it = 0, tc = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++tc) {
-        int m0, n0, kb_beg, nkb, z;
-        tile_coords(t, m0, n0, kb_beg, nkb, z);
-        const uint32_t acc = tc & 1, aph = (tc >> 1) & 1;
-        mbar_wait(&tmem_empty[acc], aph ^ 1);      // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        for (int kb = 0; kb < nkb; ++kb, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(NSPLIT >= 2 ? &ready[s] : &full[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
-          const uint32_t sb = sa + A_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            uint64_t ad = A_MN ? make_smem_desc(sa + k * 1024, BK * 128, 512, 1) : make_smem_desc(sa + k * 32, 16, 1024, 2);
-            uint64_t bd = B_MN ? make_smem_desc(sb + k * 1024, BK * 128, 512, 1) : make_smem_desc(sb + k * 32, 16, 1024, 2);
-            umma_tf32(tmem_d, ad, bd, IDESC, (kb | k) ? 1u : 0u);
-            if constexpr (NSPLIT == 3) {
-              const uint64_t lo_off = (uint64_t)(AB_BYTES >> 4);
-              umma_tf32(tmem_d, ad + lo_off, bd, IDESC, 1u);
-              umma_tf32(tmem_d, ad, bd + lo_off, IDESC, 1u);
-            }
-          }
-          umma_commit(&empty[s]);
-        }
-        umma_commit(&tmem_full[acc]);
-      }
-    }
-  } else if (NSPLIT >= 2 && warp < EPI_WARP0) {
-    // hi/lo splitter warps 2 .. 2 + SPLIT_WARPS - 1
-    const int tsp = threadIdx.x - 64;
+  } else if (warp < 4) {
+    // idle warps of the producer warpgroup
+  } else if (PREP && warp < CONS_WARP0) {
+    const int p = threadIdx.x - 128;
     uint32_t it = 0;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int m0, n0, kb_beg, nkb, z;
@@ -861,37 +669,23 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
         const int s = it % STAGES;
         const uint32_t ph = (it / STAGES) & 1;
         mbar_wait(&full[s], ph);
-        uint4* hi = reinterpret_cast<uint4*>(smem + s * STAGE_BYTES);
-        uint4* lo = reinterpret_cast<uint4*>(smem + s * STAGE_BYTES + AB_BYTES);
-#pragma unroll 4
-        for (int i = tsp; i < AB_BYTES / 16; i += SPLIT_WARPS * 32) {
-          uint4 v = hi[i];
-          uint4 h = make_uint4((v.x + 0x1000u) & 0xFFFFE000u, (v.y + 0x1000u) & 0xFFFFE000u, (v.z + 0x1000u) & 0xFFFFE000u, (v.w + 0x1000u) & 0xFFFFE000u);
-          uint4 l;
-          l.x = __float_as_uint(__uint_as_float(v.x) - __uint_as_float(h.x));
-          l.y = __float_as_uint(__uint_as_float(v.y) - __uint_as_float(h.y));
-          l.z = __float_as_uint(__uint_as_float(v.z) - __uint_as_float(h.z));
-          l.w = __float_as_uint(__uint_as_float(v.w) - __uint_as_float(h.w));
-          hi[i] = h;
-          if constexpr (NSPLIT == 3) lo[i] = l;
-        }
-        fence_proxy_async();
+        uint8_t* st = smem + s * STAGE_BYTES;
+        prep_operand<BM, A_MN, NSPLIT>(st, st + AB_BYTES, p);
+        prep_operand<BN, B_MN, NSPLIT>(st + A_BYTES, st + AB_BYTES + A_BYTES, p);
+        fence_proxy_async();     // generic-proxy smem writes -> visible to the tensor core (async proxy)
         mbar_arrive(&ready[s]);
       }
     }
-  } else if (warp >= EPI_WARP0) {
-    const int q = warp & 3;                         // TMEM lane quarter this warp may read (warp index modulo 4)
-    const int wg = (warp - EPI_WARP0) >> 2;         // epilogue warpgroup: takes the chunks c with c % EPI_WG == wg
-    const int rr = q * 32 + lane;
-    const bool elected = (threadIdx.x == (EPI_WARP0 + 4 * wg) * 32);
-    uint8_t* const wg_staging = staging + wg * EPI_STAGING_BYTES;
+  } else {
+    const int wg = (warp - CONS_WARP0) >> 2;        // consumer warpgroup: MMA rows [64 wg, 64 wg + 64); epilogue chunks c with c % 2 == wg
+    const int q = warp & 3;                         // warp inside the warpgroup
+    const int rr = q * 32 + lane;                   // epilogue row of this thread inside the tile
+    const bool elected = (threadIdx.x == (CONS_WARP0 + 4 * wg) * 32);
     const unsigned long long dseed = ep.thresh ? (*ep.seed_ptr + ep.site * 0xD1B54A32D192ED03ull) : 0ull;
     constexpr int NCHUNK = BN / 32;
-    const int last_c = ((NCHUNK - 1 - wg) / EPI_WG) * EPI_WG + wg;    // last chunk of this warpgroup
     // fused BatchNorm statistics: per-thread fp64 accumulators (lane = column of a chunk, warp = row quarter), carried ACROSS the tiles of this
-    // persistent CTA and flushed with one atomic pair per column when the CTA moves to another column block / at the end.  Flushing per
-    // tile put ~10^6 fp64 atomics per convolution onto 2 N addresses: same-address serialisation in the L2 (~10 ns each) DOUBLED the time
-    // of the memory-bound 1x1 convolutions in train mode (146 us in the step vs 67 us alone for 256 -> 64 at 64x64).
+    // persistent CTA and flushed with one atomic pair per column when the CTA moves to another column block / at the end: flushing per tile
+    // put ~10^6 fp64 atomics per convolution onto 2 N addresses, serialised in the L2.
     constexpr int NCH_WG = (NCHUNK + EPI_WG - 1) / EPI_WG;
     double racc1[NCH_WG], racc2[NCH_WG];
 #pragma unroll
@@ -907,24 +701,63 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
         }
       }
     };
-    uint32_t tc = 0, cc = 0;
-    // residual rows are prefetched one chunk ahead into registers (the first chunk of a tile before the wait for its accumulator): a load issued
-    // inside the chunk's own arithmetic exposed one DRAM latency per chunk (conv3 + identity of a bottleneck: 230 us for 603 MB)
     const bool use_res = tma_epi && ep.res != nullptr && !batched && !ep.nv_pad && (ep.opt & 1);
-    const bool use_cv = COLVEC && tma_epi && !batched && !ep.nv_pad && (ep.bias != nullptr || ep.col_scale != nullptr) && (ep.opt & 2);
-    // single-pass TF32 kernels (320 threads, 204 registers each) double-buffer the prefetch: chunk c + 1 is requested before chunk c's accumulator
-    // is read; the operand-splitting kernels (448 threads, 128 registers) re-use one buffer and request the next chunk at the end of the current one
-    constexpr bool RES_DB = (NSPLIT == 1);
-    float4 rcur[8], rnext[RES_DB ? 8 : 1];
+    const bool use_cv = tma_epi && !batched && !ep.nv_pad && (ep.bias != nullptr || ep.col_scale != nullptr) && (ep.opt & 2);
+    float4 rcur[8], rnext[8];
     int cv_n0 = -1;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++tc) {
+    uint32_t it = 0;
+    float acc[BN / 2];
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int m0, n0, kb_beg, nkb, z;
       tile_coords(t, m0, n0, kb_beg, nkb, z);
-      const uint32_t acc = tc & 1, aph = (tc >> 1) & 1;
       const int m = m0 + rr;
+      // ---- main loop: one wgmma group per k-block; the stage of k-block kb - 1 is released once its group has completed
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev_s = -1;
+      for (int kb = 0; kb < nkb; ++kb, ++it) {
+        const int s = it % STAGES;
+        const uint32_t ph = (it / STAGES) & 1;
+        mbar_wait(PREP ? &ready[s] : &full[s], ph);
+        const uint32_t sa = smem_u32(smem + s * STAGE_BYTES) + wg * (64 * 128);
+        const uint32_t sb = smem_u32(smem + s * STAGE_BYTES) + A_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / WG_K; ++k) {
+          const uint64_t ad = make_wgmma_desc(sa + k * 32), bd = make_wgmma_desc(sb + k * 32);
+          wgmma_tf32<BN>(acc, ad, bd);
+          if constexpr (NSPLIT == 3) {
+            const uint64_t lo_off = (uint64_t)(AB_BYTES >> 4);      // descriptors address in 16-byte units: the lo copies sit AB_BYTES after the hi tiles
+            wgmma_tf32<BN>(acc, ad + lo_off, bd);   // lo(A) * hi(B)
+            wgmma_tf32<BN>(acc, ad, bd + lo_off);   // hi(A) * lo(B)
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev_s >= 0 && lane == 0) mbar_arrive(&empty[prev_s]);
+        prev_s = s;
+      }
+      wgmma_wait<0>();
+      if (prev_s >= 0 && lane == 0) mbar_arrive(&empty[prev_s]);
+
+      // ---- accumulator -> staging chunks.  The TMA stores of the previous tile must have finished reading them.
       if (use_res) load_res_chunk(rcur, ep, m, n0 + wg * 32);
-      if (use_cv && n0 != cv_n0) {       // this warpgroup's chunks of the tile's column vectors -> shared memory (all its threads are past the last read)
-        const int tw = threadIdx.x - (EPI_WARP0 + 4 * wg) * 32;      // 0..127 inside the warpgroup
+      if (elected && tma_epi) tma_store_wait_read<0>();
+      cons_bar_sync();
+      {
+        // wgmma D fragment: register 4 j + {0, 1} = row (warp q) * 16 + lane / 4, columns 8 j + 2 (lane % 4) + {0, 1}; + {2, 3} = 8 rows below
+        const int r0 = wg * 64 + q * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = 8 * j + 2 * (lane & 3);
+          uint8_t* chunk = accbuf + (col >> 5) * (BM * 128);
+          const int un = (col & 31) >> 2, wo = (col & 3) << 2;
+          *reinterpret_cast<float2*>(chunk + r0 * 128 + ((un ^ (r0 & 7)) << 4) + wo) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(chunk + (r0 + 8) * 128 + ((un ^ ((r0 + 8) & 7)) << 4) + wo) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
+      if (use_cv && n0 != cv_n0) {       // this warpgroup's chunks of the tile's column vectors -> shared memory (every consumer is past the last read)
+        const int tw = threadIdx.x - (CONS_WARP0 + 4 * wg) * 32;      // 0..127 inside the warpgroup
         for (int i = tw; i < NCH_WG * 32; i += 128) {
           const int col = n0 + ((i >> 5) * EPI_WG + wg) * 32 + (i & 31);
           const bool in = col < ep.N;
@@ -935,27 +768,26 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
           colvec[BN + wg * NCH_WG * 32 + i] = add;
         }
         cv_n0 = n0;
-        epi_bar_sync(wg);
       }
-      mbar_wait(&tmem_full[acc], aph);
-      tc_fence_after();
+      cons_bar_sync();
       if (ep.stats && n0 != acc_n0) { flush_stats(); acc_n0 = n0; }
+
+      // ---- epilogue of this warpgroup's chunks: thread = row rr, 32 columns
 #pragma unroll 1
       for (int c = wg; c < NCHUNK; c += EPI_WG) {
-        if constexpr (RES_DB) {
-          if (use_res) {
-            if (c != wg) {
+        if (use_res) {
+          if (c != wg) {
 #pragma unroll
-              for (int j = 0; j < 8; ++j) rcur[j] = rnext[j];
-            }
-            if (c + EPI_WG < NCHUNK) load_res_chunk(rnext, ep, m, n0 + (c + EPI_WG) * 32);
+            for (int j = 0; j < 8; ++j) rcur[j] = rnext[j];
           }
+          if (c + EPI_WG < NCHUNK) load_res_chunk(rnext, ep, m, n0 + (c + EPI_WG) * 32);
         }
+        uint8_t* buf = accbuf + c * (BM * 128);
         float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN + c * 32), v);
-        if (c == last_c) {             // all TMEM reads of this accumulator by this thread are done: hand it back to the MMA warp
-          tc_fence_before();
-          mbar_arrive(&tmem_empty[acc]);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float4 x = *reinterpret_cast<const float4*>(buf + rr * 128 + ((j ^ (rr & 7)) << 4));
+          v[4 * j] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w;
         }
         const int nb = n0 + c * 32;
         int sc0 = nb, sc1 = 0;
@@ -967,13 +799,8 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
         if (tma_epi) {
           const float* cmul = use_cv ? colvec + (wg * NCH_WG + (c - wg) / EPI_WG) * 32 : nullptr;
           epilogue_math(v, ep, m, nb, dseed, use_res ? rcur : nullptr, cmul, use_cv ? cmul + BN : nullptr);
-          if (cc >= 2) {
-            if (elected) tma_store_wait_read<1>();
-            epi_bar_sync(wg);
-          }
-          uint8_t* buf = wg_staging + (cc & 1) * (BM * 128);
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
+          for (int j = 0; j < 8; ++j)      // back into the same (swizzled) place: the chunk is the TMA store's source
             *reinterpret_cast<float4*>(buf + rr * 128 + ((j ^ (rr & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
           fence_proxy_async();
           epi_bar_sync(wg);
@@ -997,8 +824,7 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
           if (ep.stats) {
             // fused BatchNorm statistics: column sums / sums of squares of the chunk over this warp's 32 rows.  Each lane holds one ROW
             // (32 columns) in registers: a halving butterfly over the lanes (16 + 8 + 4 + 2 + 1 = 31 exchanges per quantity) leaves lane l with
-            // the totals of column l -- no shared-memory pass (the serial 32-row LDS loop this replaces cost ~0.5 us per chunk, a third of
-            // the epilogue of the store-bound 1x1 convolutions).  Then one fp64 atomic pair per column per warp.
+            // the totals of column l.  Then one fp64 atomic pair per column per warp when the column block changes.
             const int rows_valid = min(32, ep.M - (m0 + q * 32));
             float s1[32], s2[32];
 #pragma unroll
@@ -1020,10 +846,6 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
 #pragma unroll
             for (int k = 0; k < NCH_WG; ++k) if (k == ci) { racc1[k] += (double)s1[0]; racc2[k] += (double)s2[0]; }
           }
-          ++cc;
-          if constexpr (!RES_DB) {
-            if (use_res && c + EPI_WG < NCHUNK) load_res_chunk(rcur, ep, m, n0 + (c + EPI_WG) * 32);
-          }
         } else {
 #pragma unroll
           for (int j = 0; j < 8; ++j)
@@ -1034,13 +856,7 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
     if (ep.stats) flush_stats();
     if (elected && tma_epi) tma_store_wait<0>();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-  }
 }
-
 // ---------------------------------------------------------------- host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,

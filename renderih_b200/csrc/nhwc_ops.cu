@@ -142,11 +142,12 @@ __device__ __forceinline__ BnMap bn_map(int C4) {
   BnMap m; m.q = (int)(gid % C4); m.r0 = gid / C4; m.rstride = T / C4;
   return m;
 }
-static inline int bn_grid(long long M, int C4, int threads, long long cap = 148 * 16) {
+static inline int bn_grid(long long M, int C4, int threads, long long cap = -1) {
   int g = 1, a = C4, b = threads;                 // grid must be a multiple of C4 / gcd(C4, threads)
   while (b) { int t = a % b; a = b; b = t; }
   g = C4 / a;
   long long want = (M * C4 + threads - 1) / threads;
+  if (cap < 0) cap = (long long)sm_count() * 16;
   if (want > cap) want = cap;
   if (want < 1) want = 1;
   return (int)((want + g - 1) / g * g);
@@ -157,7 +158,7 @@ RIH_API int rih_bn_colstats(const float* x, int ld, int M, int C, double* ws, cu
   RIH_REQUIRE(M > 0 && C > 0, "bn_colstats: empty");
   RIH_CUDA(cudaMemsetAsync(ws, 0, sizeof(double) * 2 * C, s));
   int gx = cdiv(C, 32);
-  int target = cdiv(148 * 8, gx);
+  int target = cdiv(sm_count() * 8, gx);
   int rows_per_cta = max(64, cdiv(M, target));
   dim3 grid(gx, cdiv(M, rows_per_cta)), block(32, 8);
   launch_k(bn_stats_kernel, grid, block, 0, s, x, ld, M, C, rows_per_cta, ws);
@@ -366,7 +367,7 @@ RIH_API int rih_bn_bwd(const float* dy, int lddy, const float* y, int ldy, const
   RIH_REQUIRE(!relu || y || relu_mask || beta, "bn_bwd: the ReLU mask needs the mask bytes, the forward output or beta");
   RIH_CUDA(cudaMemsetAsync(ws, 0, sizeof(double) * 2 * C, s));
   int gx = cdiv(C, 32);
-  int target = cdiv(148 * 8, gx);
+  int target = cdiv(sm_count() * 8, gx);
   int rows_per_cta = max(64, cdiv(M, target));
   dim3 grid(gx, cdiv(M, rows_per_cta));
   launch_k(bn_bwd_reduce_kernel, grid, 256, 0, s, dy, lddy, y, ldy, relu_mask, x, ldx, mean, rstd, gamma, beta, (int)M, C, rows_per_cta, relu, ws);
@@ -867,12 +868,12 @@ RIH_API int rih_im2col(const float* x, int ldx, float* A, int N, int H, int W, i
   const int Ho = (H + 2 * pad - R) / stride + 1, Wo = (W + 2 * pad - S) / stride + 1;
   const long long total = (long long)N * Ho * Wo * Kpad;
   if ((reinterpret_cast<uintptr_t>(A) & 15) == 0 && C == 3 && R == S && (R == 7 || R == 3)) {
-    const int g4 = (int)min((long long)148 * 32, (total / 4 + 255) / 256);
+    const int g4 = (int)min((long long)sm_count() * 32, (total / 4 + 255) / 256);
     if (R == 7) launch_k(im2col4_kernel<7, 7, 3>, g4, 256, 0, s, x, ldx, A, N, H, W, Ho, Wo, stride, pad, Kpad / 4);
     else launch_k(im2col4_kernel<3, 3, 3>, g4, 256, 0, s, x, ldx, A, N, H, W, Ho, Wo, stride, pad, Kpad / 4);
     return check_launch("im2col");
   }
-  int grid = (int)min((long long)148 * 32, (total + 255) / 256);
+  int grid = (int)min((long long)sm_count() * 32, (total + 255) / 256);
   if (R == 7 && S == 7 && C == 3) launch_k(im2col_kernel<7, 7, 3>, grid, 256, 0, s, x, ldx, A, N, H, W, C, Ho, Wo, R, S, stride, pad, Kpad);
   else if (R == 3 && S == 3 && C == 3) launch_k(im2col_kernel<3, 3, 3>, grid, 256, 0, s, x, ldx, A, N, H, W, C, Ho, Wo, R, S, stride, pad, Kpad);   // HRNet stem
   else launch_k(im2col_kernel<0, 0, 0>, grid, 256, 0, s, x, ldx, A, N, H, W, C, Ho, Wo, R, S, stride, pad, Kpad);

@@ -33,7 +33,7 @@ __global__ void layernorm_fwd_kernel(const float* __restrict__ a, int lda, const
 RIH_API int rih_layernorm_fwd(const float* a, int lda, const float* b, int ldb, const float* gamma, const float* beta,
                               float* y, int ldy, float* mean, float* rstd, int M, int F, float eps, int relu, cudaStream_t s) {
   if (M == 0) return 0;
-  int grid = min(148 * 8, cdiv(M, 8));
+  int grid = min(sm_count() * 8, cdiv(M, 8));
   launch_k(layernorm_fwd_kernel, grid, 256, 0, s, a, lda, b, ldb, gamma, beta, y, ldy, mean, rstd, M, F, eps, relu);
   return check_launch("layernorm_fwd");
 }
@@ -114,7 +114,7 @@ RIH_API int rih_layernorm_bwd(const float* dy, int lddy, const float* a, int lda
   RIH_REQUIRE(F <= 512, "layernorm_bwd: F=%d exceeds 512", F);
   if (M == 0) return 0;
 #define RIH_LN_BWD(MC, TH)                                                                                                        \
-  launch_k(layernorm_bwd_kernel<MC, TH>, min(148 * (1024 / TH), cdiv(M, TH / 32)), TH, 0, s, dy, lddy, a, lda, b, ldb, gamma, beta, mean, rstd, dx, lddx, dx_acc, \
+  launch_k(layernorm_bwd_kernel<MC, TH>, min(sm_count() * (1024 / TH), cdiv(M, TH / 32)), TH, 0, s, dy, lddy, a, lda, b, ldb, gamma, beta, mean, rstd, dx, lddx, dx_acc, \
                                                                                       dgamma, dbeta, M, F, relu)
   if (F <= 64) RIH_LN_BWD(2, 1024);
   else if (F <= 128) RIH_LN_BWD(4, 1024);
@@ -299,7 +299,7 @@ RIH_API int rih_colsum(const float* x, int ld, int M, int N, float* out, int acc
   if (!accumulate) RIH_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * N, s));
   if (M == 0) return 0;
   int gx = cdiv(N, 32);
-  int target = cdiv(148 * 4, gx);
+  int target = cdiv(sm_count() * 4, gx);
   int rows_per_cta = max(32, cdiv(M, target));
   dim3 grid(gx, cdiv(M, rows_per_cta)), block(32, 8);
   launch_k(colsum_kernel, grid, block, 0, s, x, ld, M, N, rows_per_cta, out);

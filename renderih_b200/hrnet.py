@@ -3,7 +3,7 @@
 Drop-in for the reference's `HRnet_encoder` / `hrnet_mid` (models/encoder.py:176-352) and the `HighResolutionNet` trunk
 they wrap (models/model_zoo/hrnet.py:235-527, head_type 'none').  The torch.nn modules below are PARAMETER CONTAINERS
 laid out so that `state_dict()` reproduces the reference's keys in the reference's order (released checkpoints load,
-deterministic seeded initialisation matches); their `forward` methods launch the sm_100a kernels of librih_b200.so through
+deterministic seeded initialisation matches); their `forward` methods launch the sm_90a kernels of librih_b200.so through
 `renderih_b200.ops` on NHWC row matrices [N*H*W, C].  Nothing here calls a torch convolution / normalisation kernel.
 
 Width table = `get_config` (hrnet.py:584-636): stage1 is one branch of 4 bottlenecks (64 -> 256), stages 2..4 have

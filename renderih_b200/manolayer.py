@@ -1,4 +1,4 @@
-"""B200-native drop-in for the reference's `models/manolayer.py` ManoLayer (FK + LBS), lines 100-322.
+"""H100-native drop-in for the reference's `models/manolayer.py` ManoLayer (FK + LBS), lines 100-322.
 
 Same constructor / forward contract; forward is ONE fused CUDA kernel (csrc/mano.cu).  Inputs on the CPU
 (the reference's dataset code calls the layer with CPU tensors, dataset/interhand.py:102-109) are staged to
@@ -106,7 +106,7 @@ class ManoLayer(Module):
             dev = in_dev
         else:
             if not torch.cuda.is_available():
-                raise RuntimeError('renderih_b200.ManoLayer needs a CUDA device (sm_100a); there is no CPU fallback')
+                raise RuntimeError('renderih_b200.ManoLayer needs a CUDA device (sm_90a); there is no CPU fallback')
             dev = torch.device(self._run_device or 'cuda')
         f = lambda t: None if t is None else t.to(device=dev, dtype=torch.float32)     # keeps the autograd graph
         R, P, S, T, C = f(root_rotation), f(pose), f(shape), f(trans), f(scale)

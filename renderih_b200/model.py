@@ -1,7 +1,7 @@
-"""B200-native drop-in for the reference's `models.model.HandNET_GCN` (models/model.py:18-60).
+"""H100-native drop-in for the reference's `models.model.HandNET_GCN` (models/model.py:18-60).
 
 Same constructor contract (`load_model(cfg)`), same forward signature and 4-tuple result structure, same
-1093 state_dict keys (so released checkpoints load) -- but `forward` runs hand-written sm_100a kernels from
+1093 state_dict keys (so released checkpoints load) -- but `forward` runs hand-written sm_90a kernels from
 librih_b200.so through `renderih_b200.ops`.  torch.nn modules are used ONLY as parameter containers (their
 own forward is never called); feature maps are NHWC row matrices [N*H*W, C], tokens are [B*V, F].
 """
@@ -199,7 +199,7 @@ class ResNetSimple(nn.Module):
         if not self.training and not fold_done:
             ops.bn_fold_refresh(self)        # inference: one launch folds every BatchNorm of the encoder for the conv epilogues
         if not img.requires_grad and ops.stem_supported(H, W):
-            # conv1 straight from the NCHW image: zero-bordered NHWC4 copy + tcgen05 implicit GEMM (no im2col buffer), train and eval mode
+            # conv1 straight from the NCHW image: zero-bordered NHWC4 copy + wgmma implicit GEMM (no im2col buffer), train and eval mode
             conv, bn = r.conv1, r.bn1
             fold = None if (self.training or torch.is_grad_enabled() or not ops.BN_FOLD) else bn.__dict__.get('_rih_fold')
             stats = torch.empty(2 * 64, device=img.device, dtype=torch.float64) if self.training else None
@@ -280,7 +280,7 @@ class resnet_mid(nn.Module):
 # ============================================================================ two-hand concurrency
 class HandStreams:
     """The left- and right-hand sub-graphs of a DualGraph level are independent until `inter_attn` mixes them, and each of their
-    kernels (4032 ... 16128 token rows) fills well under half of the 148 SMs.  Running them on two side streams lets the GPU overlap
+    kernels (4032 ... 16128 token rows) fills well under half of the 132 SMs of an H100.  Running them on two side streams lets the GPU overlap
     them; under CUDA-graph capture the fork/join becomes two parallel branches of the graph.  autograd replays each backward node on
     its forward stream, so the backward pass is two-stream as well.  `RIH_HAND_STREAMS=0` disables it (single stream)."""
     _cache = {}
@@ -819,7 +819,7 @@ class HandNET_GCN(nn.Module):
 
     def forward(self, img):
         if not (isinstance(img, torch.Tensor) and img.is_cuda):
-            raise RuntimeError('renderih_b200.HandNET_GCN runs only on CUDA (sm_100a) tensors; there is no CPU fallback')
+            raise RuntimeError('renderih_b200.HandNET_GCN runs only on CUDA (sm_90a) tensors; there is no CPU fallback')
         if img.dtype != torch.float32:
             raise RuntimeError('renderih_b200.HandNET_GCN expects float32 images')
         ops.seed_state.begin_forward()
@@ -899,7 +899,7 @@ class AuxStream:
         key = (device.type, device.index)
         if key not in cls._cache:
             cls._cache[key] = torch.cuda.Stream(device=device)
-            ctas = int(os.environ.get('RIH_AUX_CTAS', '72'))        # measured optimum on B200 (148 SMs): 34.7 ms sequential, 34.2 uncapped, 33.9 at 72
+            ctas = int(os.environ.get('RIH_AUX_CTAS', '72'))        # about half of the SMs; not tuned on the H100 (RIH_AUX_CTAS=0: uncapped)
             if ctas > 0:        # leave 148 - ctas SMs to the token decoder while the convolution pipeline runs
                 from ._lib import call
                 call('rih_set_stream_cta_limit', cls._cache[key].cuda_stream, ctas)

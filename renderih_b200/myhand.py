@@ -1,7 +1,7 @@
 """The `common/myhand` "graph" model variant -- what the reference's `apps/train.py` and `apps/eval_interhand.py` build by default
 (`core/lijun_trainer.py:102-113` -> `common/myhand/lijun_model_graph.load_graph_model`), SURVEY.md 8(f) row 1.
 
-Deltas against `models.model.HandNET_GCN`, all served by the same sm_100a kernels:
+Deltas against `models.model.HandNET_GCN`, all served by the same sm_90a kernels:
   * encoder: torchvision ResNet-50 trunk only, no heat-map / dense-pose heads (common/myhand/encoder_lijun.py:62-104);
   * mid: one 1x1 Conv -> ReLU -> BN per trunk level (2048 / 1024 / 512 / 256 -> 256) + global average pool (encoder_lijun.py:107-146);
   * DualGraph blocks without a Laplacian: LN -> ReLU -> Linear -> LN -> ReLU -> Linear + shortcut (model_attn/DualGraph_lijun.py:28-58);
@@ -220,7 +220,7 @@ class HandNET_GCN(nn.Module):
 
     def forward(self, img):
         if not (isinstance(img, torch.Tensor) and img.is_cuda):
-            raise RuntimeError('renderih_b200.myhand.HandNET_GCN runs only on CUDA (sm_100a) tensors; there is no CPU fallback')
+            raise RuntimeError('renderih_b200.myhand.HandNET_GCN runs only on CUDA (sm_90a) tensors; there is no CPU fallback')
         if img.dtype != torch.float32:
             raise RuntimeError('renderih_b200.myhand.HandNET_GCN expects float32 images')
         ops.seed_state.begin_forward()

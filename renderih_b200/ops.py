@@ -1,6 +1,6 @@
 """Autograd operators over the C-ABI CUDA kernels (raw pointers + current CUDA stream).
 
-Every operator here launches hand-written sm_100a kernels from librih_b200.so; torch is used only for
+Every operator here launches hand-written sm_90a kernels from librih_b200.so; torch is used only for
 memory (caching allocator), autograd bookkeeping and streams.  There is no CPU / eager fallback: tensors
 must be fp32 CUDA tensors, otherwise a RuntimeError is raised.
 """
@@ -24,7 +24,7 @@ MODE = {'conv': 'simt', 'linear': 'simt'}
 
 
 def set_gemm_mode(conv='simt', linear='simt'):
-    """Arithmetic of the GEMM-class kernels: 'simt' = exact fp32 CUDA-core path, 'tf32' = tcgen05 tensor cores with TF32
+    """Arithmetic of the GEMM-class kernels: 'simt' = exact fp32 CUDA-core path, 'tf32' = wgmma tensor cores with TF32
     multiplicands and fp32 accumulation (what the reference's cuDNN convolutions use by default on this GPU),
     'tf32c' = truncating TF32 whose mean shrinkage (7.05e-4) is compensated in the epilogue (RN-equivalent error statistics),
     'tf32rn' = TF32 with the operands rounded to nearest in shared memory before the MMA (unbiased; the cuDNN convention),
@@ -32,7 +32,7 @@ def set_gemm_mode(conv='simt', linear='simt'):
     call('rih_set_gemm_mode', GEMM_MODES[conv], GEMM_MODES[linear])
     MODE['conv'], MODE['linear'] = conv, linear
     # the attention contractions follow the nn.Linear arithmetic (the reference runs both as fp32 torch.matmul / addmm):
-    # 0 = fused SIMT kernel (exact fp32), 1 = tcgen05 TF32, 3 = tcgen05 3xTF32
+    # 0 = fused SIMT kernel (exact fp32), 1 = wgmma TF32, 3 = wgmma 3xTF32
     _ATTN['nsplit'] = {'simt': 0, 'tf32x3': 3}.get(linear, 1)
 
 
@@ -428,7 +428,7 @@ class AttnFn(Function):
 
 
 class AttnTcFn(Function):
-    """The same attention core with QK^T / PV (and the three backward contractions) on the tcgen05 tensor cores as batched per-head
+    """The same attention core with QK^T / PV (and the three backward contractions) on the wgmma tensor cores as batched per-head
     GEMMs (rih_attn_tc_fwd / rih_attn_tc_bwd); the softmax probabilities [B*H, Sq, Sk] are kept for the backward pass."""
 
     @staticmethod
@@ -1055,7 +1055,7 @@ def im2col(x, N, H, W, R, S, stride, pad, Kpad):
 
 
 class StemConvFn(Function):
-    """torchvision resnet.conv1 (7x7 / stride 2 / pad 3, 3 -> 64; models/encoder.py:108) as a tcgen05 implicit GEMM over the zero-bordered NHWC4
+    """torchvision resnet.conv1 (7x7 / stride 2 / pad 3, 3 -> 64; models/encoder.py:108) as a wgmma implicit GEMM over the zero-bordered NHWC4
     image (csrc/gemm_tc.cuh StemFwdProducer): no im2col buffer (the old path wrote and re-read 671 MB at batch 64).  w224 = the filter
     repacked [64][7][8][4].  The image receives no gradient."""
 

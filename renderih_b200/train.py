@@ -2,7 +2,7 @@
 whole-step CUDA-graph capture.
 
 Mirrors what the reference's trainer does around `network(imgTensors)` (core/lijun_trainer.py:262-313: forward,
-calc_loss_GCN, zero_grad / backward / AdamW step, DDP gradient all-reduce) with B200-first mechanics:
+calc_loss_GCN, zero_grad / backward / AdamW step, DDP gradient all-reduce) with H100-first mechanics:
   * every trainable tensor is a view of ONE flat fp32 buffer, gradients likewise -> zero_grad is one memset,
     the data-parallel exchange is ONE all-reduce of the flat gradient (155 MB) over NVLink, AdamW is one kernel;
   * BatchNorm statistics stay per rank (the reference uses no SyncBN, SURVEY.md 2.1);

@@ -35,10 +35,10 @@ def test_library_builds_and_exports_all_symbols():
     assert exported == set(_lib.parse_header()), exported ^ set(_lib.parse_header())
 
 
-def test_sass_is_sm100():
+def test_sass_is_sm90a():
     from renderih_b200 import _build
     out = subprocess.run(['cuobjdump', '-lelf', _build.build()], stdout=subprocess.PIPE).stdout.decode()
-    assert 'sm_100a' in out, out[:400]
+    assert 'sm_90a' in out, out[:400]
 
 
 def test_product_never_imports_oracle():

@@ -90,7 +90,7 @@ def test_forward_eval_matches_oracle_and_reference_golden(gold, setup):
 
 
 def test_forward_eval_tensor_core_tf32_mode(gold, setup):
-    """tcgen05 path: TF32 multiplicands (10-bit mantissa, truncated by the hardware) with fp32 accumulation for the 1x1
+    """wgmma path: TF32 multiplicands (10-bit mantissa, truncated by the hardware) with fp32 accumulation for the 1x1
     convolutions and nn.Linear GEMMs -- the arithmetic the reference's own cuDNN convolutions use on this GPU by default.
     Stated tolerance: 5e-2 relative to each tensor's max magnitude (single-pass, TRUNCATING TF32 through ~60 layers: the
     truncation bias accumulates coherently; measured 5e-4 ... 2e-2).  This mode is a speed option, not the parity mode."""
@@ -152,7 +152,7 @@ def test_forward_eval_mean_compensated_truncating_tf32(gold, setup):
 
 
 def test_forward_eval_tensor_core_3xtf32_mode(gold, setup):
-    """tcgen05 with the in-kernel hi/lo split (3 MMAs per step): fp32-faithful tensor-core arithmetic.
+    """wgmma with the in-kernel hi/lo split (3 MMAs per step): fp32-faithful tensor-core arithmetic.
     Stated tolerance: 1e-3 relative to each tensor's max magnitude (measured 3e-5 ... 4.5e-4: limited by the tensor core's
     truncating internal accumulation, two orders of magnitude tighter than single-pass TF32)."""
     from renderih_b200 import ops

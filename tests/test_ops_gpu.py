@@ -205,7 +205,7 @@ def test_attention(ops, B, H, Sq, Sk, d):
                                           (1, 2, 5, 7, 8), (2, 3, 130, 70, 32)])
 @pytest.mark.parametrize('nsplit_mode', ['tf32x3', 'tf32'])
 def test_attention_tensor_core(ops, B, H, Sq, Sk, d, nsplit_mode):
-    """tcgen05 attention core (batched per-head GEMMs over 4-D TMA maps + warp-per-row softmax), forward and backward, against plain
+    """wgmma attention core (batched per-head GEMMs over 4-D TMA maps + warp-per-row softmax), forward and backward, against plain
     torch fp32.  Stated tolerance: 3xTF32 5e-5 relative to each tensor's max (fp32-faithful), single-pass TF32 5e-3."""
     tol = 5e-5 if nsplit_mode == 'tf32x3' else 5e-3
     q, k, v = T(B * Sq, H * d, seed=1), T(B * Sk, H * d, seed=2), T(B * Sk, H * d, seed=3)
@@ -350,7 +350,7 @@ def test_no_cpu_fallback(ops):
         ops.linear(torch.randn(4, 4), torch.randn(4, 4))
 
 
-# ----------------------------------------------------------------------------- tcgen05 tensor-core GEMM (TF32 multiplicands)
+# ----------------------------------------------------------------------------- wgmma tensor-core GEMM (TF32 multiplicands)
 def _tf32_trunc(t):
     return (t.view(torch.int32) & -8192).view(torch.float32)
 
@@ -404,7 +404,7 @@ def test_gemm_tf32_splitk_bias_relu():
 @pytest.mark.parametrize('N,H,Cin,Cout,k', [(2, 64, 128, 128, 3), (4, 32, 128, 128, 3), (8, 16, 256, 256, 3), (4, 8, 512, 512, 3), (2, 64, 64, 64, 3),
                                              (2, 32, 512, 128, 1), (4, 16, 1024, 256, 1), (2, 64, 256, 64, 1)])
 def test_conv2d_tensor_core_tf32(ops, N, H, Cin, Cout, k):
-    """tcgen05 implicit-GEMM convolution (fwd, dgrad, wgrad) against fp32 torch; tolerance = single-pass TF32."""
+    """wgmma implicit-GEMM convolution (fwd, dgrad, wgrad) against fp32 torch; tolerance = single-pass TF32."""
     x = T(N, Cin, H, H)
     w = (torch.randn(Cout, Cin, k, k) * (Cin * k * k) ** -0.5).to(DEV).contiguous(memory_format=torch.channels_last).requires_grad_(True)
     xr = x.permute(0, 2, 3, 1).contiguous().reshape(N * H * H, Cin)
@@ -428,7 +428,7 @@ def test_conv2d_tensor_core_tf32(ops, N, H, Cin, Cout, k):
 @pytest.mark.parametrize('mode', ['tf32', 'tf32x3'])
 @pytest.mark.parametrize('direct', [1, 0])
 def test_conv2d_stride2_tensor_core(ops, N, H, Cin, Cout, k, mode, direct):
-    """stride-2 convolutions on the tcgen05 path.  direct = 1: the tensors are addressed in place through element-strided tensor maps (forward,
+    """stride-2 convolutions on the wgmma path.  direct = 1: the tensors are addressed in place through element-strided tensor maps (forward,
     weight gradient) and the input gradient runs as four parity-class GEMMs; direct = 0: parity-stacked input for fwd/wgrad, zero-inserted dY
     for dgrad (the copy-based formulation kept for comparison)."""
     from renderih_b200._lib import call
@@ -455,7 +455,7 @@ def test_conv2d_stride2_tensor_core(ops, N, H, Cin, Cout, k, mode, direct):
     (2, 64, 256, 48, 3, 1), (2, 64, 48, 128, 3, 1), (2, 16, 80, 208, 3, 1),                              # transition1.0 / odd multiples of 16
     (2, 64, 48, 48, 3, 2), (2, 64, 48, 96, 3, 2), (4, 32, 96, 192, 3, 2), (2, 64, 256, 96, 3, 2), (4, 16, 192, 384, 3, 2)])   # fuse / transition chains
 def test_conv2d_tensor_core_channels_multiple_of_16(ops, N, H, Cin, Cout, k, stride):
-    """Channel counts that are multiples of 16 but not of 32 / 64 (HRNet-w48: 48, 96 ...) on the tcgen05 path: the K blocks / N chunks that
+    """Channel counts that are multiples of 16 but not of 32 / 64 (HRNet-w48: 48, 96 ...) on the wgmma path: the K blocks / N chunks that
     stick out of the tensor are zero-filled (loads) and clipped (stores, 3-D dW map per tap) by the TMA unit.  3xTF32 so that any stray
     contribution would show: tolerance 1e-4 relative (fp32-faithful), forward, dgrad and wgrad; and the path must really be the tensor-core one."""
     import ctypes
@@ -588,7 +588,7 @@ def test_preprocess_u8_matches_reference_loader_ops():
 
 @pytest.mark.parametrize('mode', ['tf32', 'tf32x3'])
 def test_stem_conv_implicit_gemm(ops, mode):
-    """torchvision conv1 (7x7 / stride 2 / pad 3, 3 -> 64) as the tcgen05 implicit GEMM over the zero-bordered NHWC4 image (overlapping-stride
+    """torchvision conv1 (7x7 / stride 2 / pad 3, 3 -> 64) as the wgmma implicit GEMM over the zero-bordered NHWC4 image (overlapping-stride
     tensor map, no im2col buffer): forward, fused BatchNorm column statistics and the weight gradient against F.conv2d."""
     N, H = 2, 256
     g = torch.Generator().manual_seed(3)

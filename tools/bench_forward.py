@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""BASELINE.json configs[1]: batch-64 eval-mode forward of HandNET_GCN (encoder + attention/GCN decoder + heads) on one B200, images/s.
+"""BASELINE.json configs[1]: batch-64 eval-mode forward of HandNET_GCN (encoder + attention/GCN decoder + heads) on one H100, images/s.
 
 Companion of bench.py (which measures configs[2], the training step).  Device-timed with CUDA events over a captured CUDA graph, inputs
 resident in HBM (`value`), and end to end through the module's public call from pinned host batches with the result vertices read back
@@ -88,7 +88,7 @@ def main():
     gf = FWD_GFLOP[args.encoder]
     print(json.dumps({'metric': 'images/sec forward (eval) @batch%d 256x256' % B, 'value': B / (ms_dev * 1e-3), 'unit': 'images/s', 'n_gpus': 1,
                       'steps': args.steps, 'warmup': max(3, args.warmup), 'ms_per_step': ms_dev, 'higher_is_better': True,
-                      'dtype': 'f32 storage; tcgen05 TF32 convolutions + 3xTF32 Linear GEMMs (bench.py `ref` mode)', 'data': 'synthetic',
+                      'dtype': 'f32 storage; wgmma TF32 convolutions + 3xTF32 Linear GEMMs (bench.py `ref` mode)', 'data': 'synthetic',
                       'config': {'workload': 'BASELINE.json configs[1]: HandNET_GCN %s cfg, batch %d, 256x256, eval mode (running-stat BN folded), random-init weights, '
                                              'synthetic graph/MANO assets' % (args.encoder, B), 'cuda_graph': True,
                                  'algorithmic_gflop_per_image_fwd': gf},

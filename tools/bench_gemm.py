@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 GEMM / conv kernels on the hot shapes (CUDA events, L2 flushed between reps).
+"""Micro-benchmark of the wgmma GEMM / conv kernels on the hot shapes (CUDA events, L2 flushed between reps).
 usage: python tools/bench_gemm.py"""
 import os
 import sys

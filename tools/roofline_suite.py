@@ -56,7 +56,7 @@ run(lambda: ops.linear(t, wl, bl))
 t2 = torch.randn(B * 252, 256, device='cuda')
 wl2, bl3 = torch.randn(256, 256, device='cuda') * 0.06, torch.zeros(256, device='cuda')
 run(lambda: ops.linear(t2, wl2, bl3, res=t2))          # 256 -> 256 with bias + residual (TMA-store epilogue reading the residual rows)
-# ---- attention core on tcgen05 (forward + backward kernels)
+# ---- attention core on wgmma (forward + backward kernels)
 q = torch.randn(B * 252, 64, device='cuda', requires_grad=True)
 k = torch.randn(B * 316, 64, device='cuda', requires_grad=True)
 v = torch.randn(B * 316, 64, device='cuda', requires_grad=True)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""One small eager training step (batch 2; bench arithmetic: tcgen05 TF32 convolutions + 3xTF32 Linears / attention; hand / grid / aux / weight-gradient
+"""One small eager training step (batch 2; bench arithmetic: wgmma TF32 convolutions + 3xTF32 Linears / attention; hand / grid / aux / weight-gradient
 side streams on; fused loss; fused AdamW) for compute-sanitizer:
 
     compute-sanitizer --tool memcheck  --log-file gpurun_out/sanitizer_memcheck.log  python tools/sanitize_step.py
