@@ -11,6 +11,8 @@ Public API mirrors the reference modules it replaces:
     calc_loss_GCN / mano_loss_GCN       <-  core/Loss.py:201-277, core/Loss_mano.py:245-335 (fused mesh-term kernels, loss.py)
     Jr, batch_metrics, EvalMetrics      <-  apps/eval_interhand.py:28-170,300-552, utils/eval_metrics.py:36-50 (metrics.py)
     TrainStep, lr_at_epoch              <-  core/lijun_trainer.py:131-159,262-313, utils/lr_sc.py:159-175 (train.py)
+    mano_two_hands_renderer, rasterize, hand_mask_iou  <-  utils/vis_utils.py:153-289, utils/compute_maskiou.py:59-64,250-263 (render.py:
+                                            pytorch3d rasterise + hard Phong / ambient shading, per-sample hand mask IoU)
 """
 from . import _build
 
@@ -42,6 +44,9 @@ def __getattr__(name):
     if name in ('TrainStep', 'FlatParams', 'lr_at_epoch'):
         from . import train
         return getattr(train, name)
+    if name in ('mano_two_hands_renderer', 'rasterize', 'hand_mask_iou'):
+        from . import render
+        return getattr(render, name)
     if name in ('load_cfg', 'get_cfg_defaults'):
         from . import config
         return getattr(config, name)
