@@ -13,6 +13,9 @@ Public API mirrors the reference modules it replaces:
     TrainStep, lr_at_epoch              <-  core/lijun_trainer.py:131-159,262-313, utils/lr_sc.py:159-175 (train.py)
     mano_two_hands_renderer, rasterize, hand_mask_iou  <-  utils/vis_utils.py:153-289, utils/compute_maskiou.py:59-64,250-263 (render.py:
                                             pytorch3d rasterise + hard Phong / ambient shading, per-sample hand mask IoU)
+    NewLoss, SDF                        <-  pose_data_optimize/code_sdf/sdf_template.py:19-157, lib/sdf/sdf/sdf.py (sdf.py: two-hand
+                                            anti-penetration loss of the pose optimiser and its dense SDF grid; the function
+                                            `sdf` is renderih_b200.sdf.sdf, since the submodule owns that name)
 """
 from . import _build
 
@@ -47,6 +50,9 @@ def __getattr__(name):
     if name in ('mano_two_hands_renderer', 'rasterize', 'hand_mask_iou'):
         from . import render
         return getattr(render, name)
+    if name in ('NewLoss', 'SDF'):
+        from . import sdf as _sdf
+        return getattr(_sdf, name)
     if name in ('load_cfg', 'get_cfg_defaults'):
         from . import config
         return getattr(config, name)
