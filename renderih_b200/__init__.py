@@ -16,6 +16,8 @@ Public API mirrors the reference modules it replaces:
     NewLoss, SDF                        <-  pose_data_optimize/code_sdf/sdf_template.py:19-157, lib/sdf/sdf/sdf.py (sdf.py: two-hand
                                             anti-penetration loss of the pose optimiser and its dense SDF grid; the function
                                             `sdf` is renderih_b200.sdf.sdf, since the submodule owns that name)
+    manopth.ManoLayer                   <-  pose_data_optimize/manopth/manopth/manolayer.py (the pose optimiser's quaternion hand model,
+                                            quat/quat without PCA; a submodule only, since the top-level name ManoLayer is taken)
 """
 from . import _build
 
