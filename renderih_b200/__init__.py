@@ -18,6 +18,8 @@ Public API mirrors the reference modules it replaces:
                                             `sdf` is renderih_b200.sdf.sdf, since the submodule owns that name)
     manopth.ManoLayer                   <-  pose_data_optimize/manopth/manopth/manolayer.py (the pose optimiser's quaternion hand model,
                                             quat/quat without PCA; a submodule only, since the top-level name ManoLayer is taken)
+    geo_loss.AnchorLayer, HandPriorLoss <-  pose_data_optimize/manopth/manopth/anchorlayer.py, hocontact/postprocess/geo_loss.py (the pose
+                                            optimiser's anchor layer and its quat-norm, edge, contact and ergonomics terms for both hands)
 """
 from . import _build
 
