@@ -20,6 +20,9 @@ Public API mirrors the reference modules it replaces:
                                             quat/quat without PCA; a submodule only, since the top-level name ManoLayer is taken)
     geo_loss.AnchorLayer, HandPriorLoss <-  pose_data_optimize/manopth/manopth/anchorlayer.py, hocontact/postprocess/geo_loss.py (the pose
                                             optimiser's anchor layer and its quat-norm, edge, contact and ergonomics terms for both hands)
+    Pos2dDiscriminator, NatureLoss      <-  pose_data_optimize/Ver2Code/Discriminator/discrim.py:66-105, hocontact/postprocess/
+                                            geo_optimizer_both_batch.py:110-132 (nature.py: the pose optimiser's discriminator and its
+                                            nature loss on both hands, with the pose gradient)
 """
 from . import _build
 
@@ -57,6 +60,9 @@ def __getattr__(name):
     if name in ('NewLoss', 'SDF'):
         from . import sdf as _sdf
         return getattr(_sdf, name)
+    if name in ('Pos2dDiscriminator', 'NatureLoss'):
+        from . import nature
+        return getattr(nature, name)
     if name in ('load_cfg', 'get_cfg_defaults'):
         from . import config
         return getattr(config, name)
