@@ -23,6 +23,9 @@ Public API mirrors the reference modules it replaces:
     Pos2dDiscriminator, NatureLoss      <-  pose_data_optimize/Ver2Code/Discriminator/discrim.py:66-105, hocontact/postprocess/
                                             geo_optimizer_both_batch.py:110-132 (nature.py: the pose optimiser's discriminator and its
                                             nature loss on both hands, with the pose gradient)
+    GeOptimizer                         <-  pose_data_optimize/hocontact/postprocess/geo_optimizer_both_batch.py:22-930 (ge_optimizer.py:
+                                            the two-hand pose optimiser, set_opt_val / optimize, one CUDA graph per iteration with
+                                            device-side Adam and ReduceLROnPlateau)
 """
 from . import _build
 
@@ -63,6 +66,9 @@ def __getattr__(name):
     if name in ('Pos2dDiscriminator', 'NatureLoss'):
         from . import nature
         return getattr(nature, name)
+    if name == 'GeOptimizer':
+        from . import ge_optimizer
+        return ge_optimizer.GeOptimizer
     if name in ('load_cfg', 'get_cfg_defaults'):
         from . import config
         return getattr(config, name)

@@ -1,6 +1,7 @@
 // Token-side kernels of the DualGraph decoder: LayerNorm, Chebyshev SpMM (+[x, Lx] interleave),
 // position-embedding add (+ nearest x2 vertex upsample), column sums, dropout, global-feature broadcast.
 #include "common.cuh"
+#include "adam.cuh"
 using namespace rih;
 
 // ============================================================== LayerNorm
@@ -406,13 +407,9 @@ __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g,
                              long long n, float decay, float b1, float omb1, float b2, float omb2, float eps, float step_size, float bc2_sqrt, float gscale) {
   pdl_sync();
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    float gi = g[i] * gscale;
-    float pi = p[i] * decay;                       // decoupled weight decay: p *= 1 - lr * wd
-    float mi = b1 * m[i] + omb1 * gi;              // exp_avg.lerp_(grad, 1 - beta1)
-    float vi = b2 * v[i] + omb2 * gi * gi;         // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value = 1 - beta2)
-    m[i] = mi; v[i] = vi;
-    float denom = sqrtf(vi) / bc2_sqrt + eps;
-    p[i] = pi - step_size * (mi / denom);          // step_size = lr / (1 - beta1^t)
+    float pi = p[i], mi = m[i], vi = v[i];
+    adam_update(pi, mi, vi, g[i] * gscale, decay, b1, omb1, b2, omb2, eps, step_size, bc2_sqrt);
+    p[i] = pi; m[i] = mi; v[i] = vi;
   }
 }
 // torch.optim.AdamW.step (single-tensor path of torch/optim/adamw.py): every scalar (1 - beta, the bias corrections, lr / bc1, 1 - lr * wd) is
