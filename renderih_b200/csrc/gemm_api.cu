@@ -15,6 +15,7 @@ void set_narrow_small(int on);
 void set_wgrad_wide(int on);
 void set_s2_direct(int on);
 void set_tma_res(int on);
+void set_gemm_rs(int on);
 void set_epilogue_opt(int v);
 void set_tma_grouped(int on);
 int s2_direct();
@@ -69,6 +70,10 @@ RIH_API int rih_set_epilogue_opt(int bits) { tc::set_epilogue_opt(bits); return 
 RIH_API int rih_set_tma_res(int on) { tc::set_tma_res(on); return 0; }
 RIH_API int rih_set_s2_direct(int on) { tc::set_s2_direct(on); return 0; }
 RIH_API int rih_set_wgrad_wide(int on) { tc::set_wgrad_wide(on); return 0; }
+// 1 (default) = the tensor-core convolution weight gradients (rih_conv2d_wgrad, rih_stem_conv_wgrad) read their MN-major dY operand from
+// shared memory into registers and multiply it with the register-A form of wgmma; only the input operand is transposed in shared memory.
+// 0 = both operands are transposed in shared memory by the preparation warpgroup.  Results are bitwise identical.
+RIH_API int rih_set_gemm_rs(int on) { tc::set_gemm_rs(on); return 0; }
 static inline bool use_tc(int which) {
   if (g_mode[which] == 0) return false;
   tc::set_nsplit(g_mode[which] == 2 ? 3 : (g_mode[which] == 3 ? 2 : 1));

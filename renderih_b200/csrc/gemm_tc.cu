@@ -151,9 +151,11 @@ static int g_tma_grouped = 7;    // grouped rank-3 tensor maps for MN-major oper
 void set_tma_grouped(int on) { g_tma_grouped = on & 7; }       // bit 0: rank-3 grouped maps for dense MN-major operands / dY, bit 1: rank-5 grouped input maps of the conv wgrad, bit 2: grouped weight boxes of the conv dgrad
 static int g_epi_opt = 7;        // Epilogue::opt of every launch (rih_set_epilogue_opt)
 void set_epilogue_opt(int v) { g_epi_opt = v & 7; }
+static int g_gemm_rs = 1;        // MN-major A operands of the convolution weight gradients read into registers by the consumers (rih_set_gemm_rs)
+void set_gemm_rs(int on) { g_gemm_rs = on ? 1 : 0; }
 static int g_tma_res = 1;        // residual rows read by the TMA-store epilogue (0: GEMMs with a residual use per-thread global stores, as before)
 void set_tma_res(int on) { g_tma_res = on ? 1 : 0; }
-template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT>
+template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT, bool A_RS>
 static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep, const Producer& prod, int M, int N, int num_kb, int splits,
                       int kb_per_split, cudaStream_t s, const CUtensorMap* c_map = nullptr) {
   // TMA-store epilogue whenever the output is a 16-byte aligned matrix (a residual is read back row-wise by the epilogue threads when it is aligned too)
@@ -172,7 +174,7 @@ static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep,
   }
   if (ep.col_scale && ep.bias) { set_error("gemm_tc: a folded per-column affine and a bias cannot be combined (fold the bias into the shift)"); return 1; }
   g_launch_counts[tma_epi ? 0 : 1]++;
-  auto pk = gemm_tc_persistent_kernel<BN, A_MN, B_MN, Producer, NSPLIT>;
+  auto pk = gemm_tc_persistent_kernel<BN, A_MN, B_MN, Producer, NSPLIT, A_RS>;
   static bool pattr = false;
   if (!pattr) {
     if (cudaFuncSetAttribute(pk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<BN, NSPLIT>()) != cudaSuccess) {
@@ -188,14 +190,14 @@ static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep,
   const int ctas = (int)(total < cap ? total : cap);
   if (ep.stats && !(g_persistent && tma_epi && splits == 1)) ep.stats = nullptr;
   g_stats_fused = ep.stats != nullptr;
-  launch_k(pk, dim3(ctas), dim3(persistent_threads<A_MN, B_MN, NSPLIT>()), (size_t)smem_bytes<BN, NSPLIT>(), s, ta, tb, tc_, ep, prod, num_kb, kb_per_split,
+  launch_k(pk, dim3(ctas), dim3(persistent_threads<A_MN, B_MN, NSPLIT, A_RS>()), (size_t)smem_bytes<BN, NSPLIT>(), s, ta, tb, tc_, ep, prod, num_kb, kb_per_split,
            tiles_m, tiles_n, splits, tma_epi);
   return check_launch(g_persistent ? "gemm_tc_persistent" : "gemm_tc");
 }
 static int g_nsplit = 1;   // set per call by the dispatchers below (1 = TF32, 2 = TF32 rn, 3 = 3xTF32)
 static float g_scale = 1.f; // accumulator scale (bias-compensated truncating TF32)
 void set_acc_scale(float s) { g_scale = s; }
-template <int BN, bool A_MN, bool B_MN, class Producer>
+template <int BN, bool A_MN, bool B_MN, class Producer, bool A_RS = false>
 static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep, const Producer& prod, int M, int N, int num_kb, int splits,
                       int kb_per_split, cudaStream_t s, const CUtensorMap* c_map = nullptr) {
   ep.scale = g_scale;
@@ -203,9 +205,9 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep,
   ep.kb_rotate = g_kb_rotate;
   ep.a_policy = g_l2_hints ? 1ull : 0ull;
   ep.opt = g_epi_opt;
-  if (g_nsplit == 3) return launch_one<BN, A_MN, B_MN, Producer, 3>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
-  if (g_nsplit == 2) return launch_one<BN, A_MN, B_MN, Producer, 2>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
-  return launch_one<BN, A_MN, B_MN, Producer, 1>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
+  if (g_nsplit == 3) return launch_one<BN, A_MN, B_MN, Producer, 3, A_RS>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
+  if (g_nsplit == 2) return launch_one<BN, A_MN, B_MN, Producer, 2, A_RS>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
+  return launch_one<BN, A_MN, B_MN, Producer, 1, A_RS>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
 }
 void set_nsplit(int n) { g_nsplit = (n == 3) ? 3 : (n == 2 ? 2 : 1); }
 
@@ -469,6 +471,7 @@ int stem_wgrad_tf32(const float* dy, int lddy, const float* xp, Epilogue ep, int
   int num_kb = P / BK, splits, kps;
   plan_splitk(ep, 64, 224, 128, num_kb, 1, splits, kps, s);
   StemWgradProducer<128> p{Ho, Wo};
+  if (g_gemm_rs) return launch_cfg<128, true, true, StemWgradProducer<128>, true>(ta, tb, ep, p, 64, 224, num_kb, splits, kps, s);
   return launch_cfg<128, true, true>(ta, tb, ep, p, 64, 224, num_kb, splits, kps, s);
 }
 
@@ -516,8 +519,13 @@ int conv_wgrad_tf32(const float* dy, const float* x, Epilogue ep, const ConvGeom
     if (make_tmap_wgrad_out(&tcm, ep.c, g.Cout, taps, g.Cin)) return 1;
     cmap = &tcm; ep.nv_pad = cin_pad; ep.nv_real = g.Cin;
   }
-  if (BN == 128) { ConvWgradProducer<128> p{cg, a_grp, wide ? b_grp : 0}; return launch_cfg<128, true, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap); }
+  if (BN == 128) {
+    ConvWgradProducer<128> p{cg, a_grp, wide ? b_grp : 0};
+    if (g_gemm_rs) return launch_cfg<128, true, true, ConvWgradProducer<128>, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap);
+    return launch_cfg<128, true, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap);
+  }
   ConvWgradProducer<64> p{cg, a_grp, 0};
+  if (g_gemm_rs) return launch_cfg<64, true, true, ConvWgradProducer<64>, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap);
   return launch_cfg<64, true, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap);
 }
 

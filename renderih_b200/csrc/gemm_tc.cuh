@@ -4,8 +4,9 @@
 // Operand tiles are [rows x 128 bytes] TMA boxes with SWIZZLE_128B; the same box format serves
 //   K-major  operands (rows = M/N index, 32 consecutive k per row)          and
 //   MN-major operands (rows = k index, 32 consecutive m/n per row; one box per 32-wide m/n chunk).
-// wgmma reads TF32 operands K-major only, so MN-major tiles are transposed in shared memory by a preparation warpgroup (which also
-// rounds / splits the operands of the TF32-rn and 3xTF32 kernels) before the consumers multiply them.
+// wgmma reads TF32 shared-memory operands K-major only, so MN-major tiles are transposed in shared memory by a preparation warpgroup (which
+// also rounds / splits the operands of the TF32-rn and 3xTF32 kernels) before the consumers multiply them -- except an MN-major A tile of an
+// A_RS kernel, which the consumers load into registers for the register-A form of wgmma.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -150,6 +151,22 @@ template <> __device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint
       "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc) : "memory");
+}
+// The same with A (64 x 8) from registers: per thread a[0..3] = rows (warp q) * 16 + lane / 4 + {0, 8, 0, 8}, k = lane % 4 + {0, 0, 4, 4}
+template <int BN> __device__ __forceinline__ void wgmma_tf32_rs(float (&d)[BN / 2], const uint32_t (&a)[4], uint64_t bdesc);
+template <> __device__ __forceinline__ void wgmma_tf32_rs<64>(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc) : "memory");
+}
+template <> __device__ __forceinline__ void wgmma_tf32_rs<128>(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc) : "memory");
 }
 
 // NSPLIT = 1: single-pass TF32 (the tensor core ignores the low mantissa bits of the fp32 operands).  NSPLIT = 2: single-pass TF32 with the
@@ -567,25 +584,72 @@ __device__ __forceinline__ void prep_operand(uint8_t* hi, uint8_t* lo, int p) {
   }
 }
 
+// ---------------------------------------------------------------- register-A operand (A_RS kernels)
+// An MN-major A tile is not transposed in shared memory: each consumer thread loads its wgmma A fragment straight from the BM / 32 TMA chunks
+// of [32 k rows x 128 B] with ld.shared.  Warp q of consumer warpgroup wg owns tile rows m = 64 wg + 16 q + g + {0, 8} (g = lane / 4), and
+// per k8 step ks the k = 8 ks + t + {0, 4} (t = lane % 4).
+// Banks: element (k, m) is word 32 k + 4 ((m' >> 2) ^ (k & 7)) + (m' & 3) of chunk m / 32, m' = m % 32 = 16 (q & 1) + g (+ 8).  If every lane
+// loaded the same one of its two k, the warp would cover m' >> 2 in {4h, 4h + 1} (+ 2) and k & 7 = t in 0..3: 4 distinct 16-byte units,
+// 16 banks, 2-way conflicts.  So lanes 16..31 (g >= 4) load their k + 4 element first and lanes 0..15 their k element: the two halves of the
+// warp then hit the two disjoint unit groups (k & 7 < 4 and k & 7 >= 4), every 32-bit load is conflict-free (one wavefront per warp and
+// load), and two selects per row put the values back into fragment order.
+struct RsFrag {
+  uint32_t off[4];   // byte offsets in the stage for k step 0: (row g, first k), (row g, second k), (row g + 8, first k), (row g + 8, second k)
+  bool swap;         // lanes 16..31: the first load is k + 4
+  __device__ __forceinline__ void init(int wg, int q, int lane) {
+    const int g = lane >> 2, t = lane & 3, hsel = lane >> 4;
+    const uint32_t chunk = (uint32_t)(2 * wg + (q >> 1)) * (BK * 128);
+    swap = hsel != 0;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int mm = 16 * (q & 1) + g + 8 * r;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int k = t + 4 * (i ^ hsel);
+        off[2 * r + i] = chunk + k * 128 + ((((mm >> 2) ^ (k & 7)) << 4) | ((mm & 3) << 2));
+      }
+    }
+  }
+  // fragment of k step ks (8 k rows = 1024 B further; k & 7 and so the swizzle are unchanged) from the A tile at `st`
+  __device__ __forceinline__ void load(uint32_t (&a)[4], const uint8_t* st, int ks) const {
+    uint32_t x[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) x[i] = *reinterpret_cast<const uint32_t*>(st + off[i] + ks * 1024);
+    a[0] = swap ? x[1] : x[0]; a[2] = swap ? x[0] : x[1];
+    a[1] = swap ? x[3] : x[2]; a[3] = swap ? x[2] : x[3];
+  }
+};
+// register form of split_tf32: the same rounding (NSPLIT >= 2) and hi / lo split (NSPLIT == 3) of one A fragment
+template <int NSPLIT> __device__ __forceinline__ void split_frag(const uint32_t (&a)[4], uint32_t (&h)[4], uint32_t (&l)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    h[i] = NSPLIT == 1 ? a[i] : ((a[i] + 0x1000u) & 0xFFFFE000u);
+    if constexpr (NSPLIT == 3) l[i] = __float_as_uint(__uint_as_float(a[i]) - __uint_as_float(h[i]));
+  }
+}
+
 // ---------------------------------------------------------------- the kernel
 // Persistent: the grid is at most one CTA per SM and loops over output tiles (static round-robin); a grid of one CTA per tile is the
 // non-persistent form.  The shared-memory stage ring runs continuously across tiles, so the TMA loads of tile i+1 overlap the epilogue of tile i.
 //   warpgroup 0: warp 0 = TMA producer (warps 1-3 idle)
-//   warpgroup 1 (only when an operand is MN-major or NSPLIT >= 2): operand preparation (prep_operand)
+//   warpgroup 1 (only when an operand needs a transpose, rounding or a split in shared memory): operand preparation (prep_operand)
 //   last two warpgroups: consumers -- wgmma over rows [64 wg, 64 wg + 64) of the tile, then the epilogue of the chunks c with c % 2 == wg
+// A_RS (MN-major A only): the consumers read A from the TMA chunks into registers (RsFrag) and round / split it there; the preparation
+// warpgroup handles B alone and is dropped when B needs nothing.
 // tma_epi != 0: the epilogue writes 32-column chunks with TMA stores (cp.reduce.async.bulk ... .add for accumulate / split-K), fully coalesced
 // and clipped at the tensor edge by the hardware.
-template <bool A_MN, bool B_MN, int NSPLIT> __host__ __device__ constexpr bool has_prep() { return A_MN || B_MN || NSPLIT >= 2; }
-template <bool A_MN, bool B_MN, int NSPLIT> __host__ __device__ constexpr int persistent_threads() { return (has_prep<A_MN, B_MN, NSPLIT>() ? 4 : 3) * 128; }
+template <bool A_MN, bool B_MN, int NSPLIT, bool A_RS = false> __host__ __device__ constexpr bool has_prep() { return (A_MN && !A_RS) || B_MN || NSPLIT >= 2; }
+template <bool A_MN, bool B_MN, int NSPLIT, bool A_RS = false> __host__ __device__ constexpr int persistent_threads() { return (has_prep<A_MN, B_MN, NSPLIT, A_RS>() ? 4 : 3) * 128; }
 
-template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT>
-__global__ void __launch_bounds__(persistent_threads<A_MN, B_MN, NSPLIT>(), 1)
+template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT, bool A_RS = false>
+__global__ void __launch_bounds__(persistent_threads<A_MN, B_MN, NSPLIT, A_RS>(), 1)
 gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_c,
                           Epilogue ep, Producer prod, int num_kb_total, int kb_per_split, int tiles_m, int tiles_n, int splits, int tma_epi) {
   constexpr int STAGES = num_stages<BN, NSPLIT>();
   constexpr int A_BYTES = BM * 128, B_BYTES = BN * 128, AB_BYTES = A_BYTES + B_BYTES;
   constexpr int STAGE_BYTES = stage_bytes<BN, NSPLIT>();
-  constexpr bool PREP = has_prep<A_MN, B_MN, NSPLIT>();
+  static_assert(!A_RS || A_MN, "the register-A main loop reads MN-major A tiles");
+  constexpr bool PREP = has_prep<A_MN, B_MN, NSPLIT, A_RS>();
   constexpr int CONS_WARP0 = PREP ? 8 : 4;
   constexpr int EPI_WG = 2;
   extern __shared__ uint8_t smem_raw[];
@@ -670,7 +734,7 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
         const uint32_t ph = (it / STAGES) & 1;
         mbar_wait(&full[s], ph);
         uint8_t* st = smem + s * STAGE_BYTES;
-        prep_operand<BM, A_MN, NSPLIT>(st, st + AB_BYTES, p);
+        if constexpr (!A_RS) prep_operand<BM, A_MN, NSPLIT>(st, st + AB_BYTES, p);
         prep_operand<BN, B_MN, NSPLIT>(st + A_BYTES, st + AB_BYTES + A_BYTES, p);
         fence_proxy_async();     // generic-proxy smem writes -> visible to the tensor core (async proxy)
         mbar_arrive(&ready[s]);
@@ -707,35 +771,71 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
     int cv_n0 = -1;
     uint32_t it = 0;
     float acc[BN / 2];
+    RsFrag frag;
+    if constexpr (A_RS) frag.init(wg, q, lane);
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int m0, n0, kb_beg, nkb, z;
       tile_coords(t, m0, n0, kb_beg, nkb, z);
       const int m = m0 + rr;
-      // ---- main loop: one wgmma group per k-block; the stage of k-block kb - 1 is released once its group has completed
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       int prev_s = -1;
-      for (int kb = 0; kb < nkb; ++kb, ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        mbar_wait(PREP ? &ready[s] : &full[s], ph);
-        const uint32_t sa = smem_u32(smem + s * STAGE_BYTES) + wg * (64 * 128);
-        const uint32_t sb = smem_u32(smem + s * STAGE_BYTES) + A_BYTES;
-        wgmma_fence();
+      if constexpr (A_RS) {
+        // ---- register-A main loop: one wgmma group per k8 step; the fragments alternate between two register sets (ahi / alo [ks & 1]).
+        // Before a set is reloaded, wgmma_wait<1> retires the group that read it two steps earlier, so one group stays in flight while the
+        // next fragment loads.  The stage of k-block kb - 1 is released at step 1 of k-block kb: by then its last group has completed, and
+        // so have all of its fragment loads, which every lane finished before the warpgroup issued the group.
+        constexpr int KS = BK / WG_K;
+        uint32_t ahi[2][4], alo[2][4];
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+          const int s = it % STAGES;
+          const uint32_t ph = (it / STAGES) & 1;
+          if constexpr (PREP) mbar_wait(&ready[s], ph);     // B prepared
+          mbar_wait(&full[s], ph);                          // A landed (already observed through ready[s] when PREP)
+          const uint8_t* st = smem + s * STAGE_BYTES;
+          const uint32_t sb = smem_u32(st) + A_BYTES;
 #pragma unroll
-        for (int k = 0; k < BK / WG_K; ++k) {
-          const uint64_t ad = make_wgmma_desc(sa + k * 32), bd = make_wgmma_desc(sb + k * 32);
-          wgmma_tf32<BN>(acc, ad, bd);
-          if constexpr (NSPLIT == 3) {
-            const uint64_t lo_off = (uint64_t)(AB_BYTES >> 4);      // descriptors address in 16-byte units: the lo copies sit AB_BYTES after the hi tiles
-            wgmma_tf32<BN>(acc, ad + lo_off, bd);   // lo(A) * hi(B)
-            wgmma_tf32<BN>(acc, ad, bd + lo_off);   // hi(A) * lo(B)
+          for (int ks = 0; ks < KS; ++ks) {
+            wgmma_wait<1>();
+            if (ks == 1 && prev_s >= 0 && lane == 0) mbar_arrive(&empty[prev_s]);
+            uint32_t a[4];
+            frag.load(a, st, ks);
+            split_frag<NSPLIT>(a, ahi[ks & 1], alo[ks & 1]);
+            wgmma_fence();
+            const uint64_t bd = make_wgmma_desc(sb + ks * 32);
+            wgmma_tf32_rs<BN>(acc, ahi[ks & 1], bd);
+            if constexpr (NSPLIT == 3) {
+              wgmma_tf32_rs<BN>(acc, alo[ks & 1], bd);                              // lo(A) * hi(B)
+              wgmma_tf32_rs<BN>(acc, ahi[ks & 1], bd + (uint64_t)(AB_BYTES >> 4));  // hi(A) * lo(B)
+            }
+            wgmma_commit();
           }
+          prev_s = s;
         }
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (prev_s >= 0 && lane == 0) mbar_arrive(&empty[prev_s]);
-        prev_s = s;
+      } else {
+        // ---- main loop: one wgmma group per k-block; the stage of k-block kb - 1 is released once its group has completed
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+          const int s = it % STAGES;
+          const uint32_t ph = (it / STAGES) & 1;
+          mbar_wait(PREP ? &ready[s] : &full[s], ph);
+          const uint32_t sa = smem_u32(smem + s * STAGE_BYTES) + wg * (64 * 128);
+          const uint32_t sb = smem_u32(smem + s * STAGE_BYTES) + A_BYTES;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / WG_K; ++k) {
+            const uint64_t ad = make_wgmma_desc(sa + k * 32), bd = make_wgmma_desc(sb + k * 32);
+            wgmma_tf32<BN>(acc, ad, bd);
+            if constexpr (NSPLIT == 3) {
+              const uint64_t lo_off = (uint64_t)(AB_BYTES >> 4);      // descriptors address in 16-byte units: the lo copies sit AB_BYTES after the hi tiles
+              wgmma_tf32<BN>(acc, ad + lo_off, bd);   // lo(A) * hi(B)
+              wgmma_tf32<BN>(acc, ad, bd + lo_off);   // hi(A) * lo(B)
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev_s >= 0 && lane == 0) mbar_arrive(&empty[prev_s]);
+          prev_s = s;
+        }
       }
       wgmma_wait<0>();
       if (prev_s >= 0 && lane == 0) mbar_arrive(&empty[prev_s]);
