@@ -15,12 +15,13 @@ void set_narrow_small(int on);
 void set_wgrad_wide(int on);
 void set_s2_direct(int on);
 void set_tma_res(int on);
-void set_gemm_rs(int on);
+void set_gemm_rs(int bits);
 void set_epilogue_opt(int v);
 void set_tma_grouped(int on);
 int s2_direct();
 void set_acc_scale(float s);
 extern int g_stats_fused;
+extern long long g_dgrad_t_launches;
 long long conv_tc_workspace(const ConvGeom& g, int which);
 int conv_fwd_tf32(const float* x, const float* w, Epilogue ep, const ConvGeom& g, float* ws, cudaStream_t s);
 int conv_dgrad_tf32(const float* dy, const float* w, Epilogue ep, const ConvGeom& g, float* ws, cudaStream_t s);
@@ -65,15 +66,27 @@ RIH_API int rih_gemm_launch_counts(long long* out, int reset) {
   if (reset) for (int i = 0; i < 3; ++i) tc::g_launch_counts[i] = 0;
   return 0;
 }
+// *out = transposed-output input-gradient launches (rih_set_gemm_rs bit 1) since the last reset; reset != 0 zeroes the count afterwards
+RIH_API int rih_gemm_dgrad_t_launches(long long* out, int reset) {
+  if (out) *out = tc::g_dgrad_t_launches;
+  if (reset) tc::g_dgrad_t_launches = 0;
+  return 0;
+}
 RIH_API int rih_set_tma_grouped(int on) { tc::set_tma_grouped(on); return 0; }
 RIH_API int rih_set_epilogue_opt(int bits) { tc::set_epilogue_opt(bits); return 0; }
 RIH_API int rih_set_tma_res(int on) { tc::set_tma_res(on); return 0; }
 RIH_API int rih_set_s2_direct(int on) { tc::set_s2_direct(on); return 0; }
 RIH_API int rih_set_wgrad_wide(int on) { tc::set_wgrad_wide(on); return 0; }
-// 1 (default) = the tensor-core convolution weight gradients (rih_conv2d_wgrad, rih_stem_conv_wgrad) read their MN-major dY operand from
-// shared memory into registers and multiply it with the register-A form of wgmma; only the input operand is transposed in shared memory.
-// 0 = both operands are transposed in shared memory by the preparation warpgroup.  Results are bitwise identical.
-RIH_API int rih_set_gemm_rs(int on) { tc::set_gemm_rs(on); return 0; }
+// Bit mask of the register-A main loops of the wgmma GEMM (default 3):
+//   bit 0: the 3x3 / strided convolution weight gradients and the stem's (rih_conv2d_wgrad, rih_stem_conv_wgrad) read their MN-major dY operand
+//          from shared memory into registers and multiply it with the register-A form of wgmma; only the input operand is transposed in shared memory.
+//   bit 1: the input gradients with at least 128 input channels / in-features (rih_conv2d_dgrad, rih_linear_dgrad) are computed transposed,
+//          dX^T = W^T dY^T: the weights are read into registers and dY is a K-major operand, so nothing is transposed in shared memory and the
+//          TF32 convolution kernels drop the preparation warpgroup.  Every other MN-major A operand (1x1 convolution and Linear weight gradients,
+//          attention dK / dV) is read into registers too.
+// Cleared bits select the shared-memory transpose by the preparation warpgroup (rih_set_gemm_rs(1) = the kernel choices before bit 1 existed).
+// Same products in the same k order: results agree bitwise or to fp32 reordering of the accumulation.
+RIH_API int rih_set_gemm_rs(int bits) { tc::set_gemm_rs(bits); return 0; }
 static inline bool use_tc(int which) {
   if (g_mode[which] == 0) return false;
   tc::set_nsplit(g_mode[which] == 2 ? 3 : (g_mode[which] == 3 ? 2 : 1));

@@ -146,16 +146,18 @@ static int g_persistent = 1;     // 0 = one CTA per tile (non-persistent kernel;
 void set_persistent(int on) { g_persistent = on ? 1 : 0; }
 static int g_tma_epilogue = 1;   // 0 = per-thread global stores (debug / comparison)
 void set_tma_epilogue(int on) { g_tma_epilogue = on ? 1 : 0; }
-long long g_launch_counts[3] = {0, 0, 0};   // tensor-core launches with the TMA-store epilogue / with per-thread stores / SIMT GEMM launches (rih_gemm_launch_counts)
+long long g_launch_counts[3] = {0, 0, 0};
+long long g_dgrad_t_launches = 0;           // transposed-output (OUT_T) launches (rih_gemm_dgrad_t_launches)   // tensor-core launches with the TMA-store epilogue / with per-thread stores / SIMT GEMM launches (rih_gemm_launch_counts)
 static int g_tma_grouped = 7;    // grouped rank-3 tensor maps for MN-major operands (rih_set_tma_grouped)
 void set_tma_grouped(int on) { g_tma_grouped = on & 7; }       // bit 0: rank-3 grouped maps for dense MN-major operands / dY, bit 1: rank-5 grouped input maps of the conv wgrad, bit 2: grouped weight boxes of the conv dgrad
 static int g_epi_opt = 7;        // Epilogue::opt of every launch (rih_set_epilogue_opt)
 void set_epilogue_opt(int v) { g_epi_opt = v & 7; }
-static int g_gemm_rs = 1;        // MN-major A operands of the convolution weight gradients read into registers by the consumers (rih_set_gemm_rs)
-void set_gemm_rs(int on) { g_gemm_rs = on ? 1 : 0; }
+static int g_gemm_rs = 3;        // register-A main loops (rih_set_gemm_rs): bit 0 = the 3x3 / strided convolution weight gradients and the stem's,
+                                 // bit 1 = transposed-output input gradients (dgrad_t) and every other MN-major A operand (dense and batched)
+void set_gemm_rs(int bits) { g_gemm_rs = bits & 3; }
 static int g_tma_res = 1;        // residual rows read by the TMA-store epilogue (0: GEMMs with a residual use per-thread global stores, as before)
 void set_tma_res(int on) { g_tma_res = on ? 1 : 0; }
-template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT, bool A_RS>
+template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT, bool A_RS, bool OUT_T>
 static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep, const Producer& prod, int M, int N, int num_kb, int splits,
                       int kb_per_split, cudaStream_t s, const CUtensorMap* c_map = nullptr) {
   // TMA-store epilogue whenever the output is a 16-byte aligned matrix (a residual is read back row-wise by the epilogue threads when it is aligned too)
@@ -173,8 +175,14 @@ static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep,
     tc_ = ta;
   }
   if (ep.col_scale && ep.bias) { set_error("gemm_tc: a folded per-column affine and a bias cannot be combined (fold the bias into the shift)"); return 1; }
+  if (OUT_T && (!c_map || ep.bias || ep.relu || ep.res || ep.stats || ep.thresh || ep.col_scale || ep.relu_post || ep.mode > 1 || ep.nv_pad ||
+                ep.batch_heads || splits != 1)) {
+    set_error("gemm_tc: the transposed-output epilogue only scales and stores / accumulates (no bias, activation, residual, dropout, statistics, split-K)");
+    return 1;
+  }
   g_launch_counts[tma_epi ? 0 : 1]++;
-  auto pk = gemm_tc_persistent_kernel<BN, A_MN, B_MN, Producer, NSPLIT, A_RS>;
+  if (OUT_T) g_dgrad_t_launches++;
+  auto pk = gemm_tc_persistent_kernel<BN, A_MN, B_MN, Producer, NSPLIT, A_RS, OUT_T>;
   static bool pattr = false;
   if (!pattr) {
     if (cudaFuncSetAttribute(pk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<BN, NSPLIT>()) != cudaSuccess) {
@@ -197,7 +205,7 @@ static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep,
 static int g_nsplit = 1;   // set per call by the dispatchers below (1 = TF32, 2 = TF32 rn, 3 = 3xTF32)
 static float g_scale = 1.f; // accumulator scale (bias-compensated truncating TF32)
 void set_acc_scale(float s) { g_scale = s; }
-template <int BN, bool A_MN, bool B_MN, class Producer, bool A_RS = false>
+template <int BN, bool A_MN, bool B_MN, class Producer, bool A_RS = false, bool OUT_T = false>
 static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep, const Producer& prod, int M, int N, int num_kb, int splits,
                       int kb_per_split, cudaStream_t s, const CUtensorMap* c_map = nullptr) {
   ep.scale = g_scale;
@@ -205,9 +213,9 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep,
   ep.kb_rotate = g_kb_rotate;
   ep.a_policy = g_l2_hints ? 1ull : 0ull;
   ep.opt = g_epi_opt;
-  if (g_nsplit == 3) return launch_one<BN, A_MN, B_MN, Producer, 3, A_RS>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
-  if (g_nsplit == 2) return launch_one<BN, A_MN, B_MN, Producer, 2, A_RS>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
-  return launch_one<BN, A_MN, B_MN, Producer, 1, A_RS>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
+  if (g_nsplit == 3) return launch_one<BN, A_MN, B_MN, Producer, 3, A_RS, OUT_T>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
+  if (g_nsplit == 2) return launch_one<BN, A_MN, B_MN, Producer, 2, A_RS, OUT_T>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
+  return launch_one<BN, A_MN, B_MN, Producer, 1, A_RS, OUT_T>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
 }
 void set_nsplit(int n) { g_nsplit = (n == 3) ? 3 : (n == 2 ? 2 : 1); }
 
@@ -234,10 +242,33 @@ static void plan_splitk(Epilogue& ep, int M, int N, int BN, int num_kb, int allo
   }
 }
 
+// Transposed-output input gradients (rih_set_gemm_rs bit 1): c[rows, cols] (+)= dY . W computed as c^T = W^T dY^T, so that the weights are
+// an MN-major A operand read into registers and dY a K-major B operand (see OUT_T in gemm_tc.cuh).  The 128 rows of such a tile are output
+// columns (input channels / in-features): narrower outputs would leave rows empty and keep the untransposed product (measured per shape:
+// tools/bench_dgrad.py).  The epilogue of the transposed form only scales and stores / accumulates into a 16-byte aligned output.
+static bool dgrad_t(const Epilogue& ep, int cols) {
+  return (g_gemm_rs & 2) && g_persistent && g_tma_epilogue && cols >= 128 &&
+         ep.mode <= 1 && !ep.bias && !ep.relu && !ep.res && !ep.stats && !ep.thresh && !ep.col_scale && !ep.relu_post &&
+         (reinterpret_cast<uintptr_t>(ep.c) & 15) == 0 && ep.ldc % 4 == 0;
+}
+
+// c[M, N] (+)= a[M, K] . b[K, N] (a K-major, b MN-major) as c^T = b^T a^T: b is the MN-major A operand of a register-A, transposed-output launch
+static int gemm_tf32_t(const float* a, long long lda, const float* b, long long ldb, Epilogue ep, int M, int N, int K, cudaStream_t s) {
+  CUtensorMap ta, tb, tcm;
+  const int a_grp = ((g_tma_grouped & 1) && N % 32 == 0) ? 1 : 0;
+  if (a_grp ? make_tmap_2d_grouped(&ta, b, K, N, ldb, BM / 32) : make_tmap_2d(&ta, b, K, N, ldb, 32, true)) return 1;
+  if (make_tmap_2d(&tb, a, M, K, lda, 128)) return 1;
+  if (make_tmap_2d(&tcm, ep.c, M, N, ep.ldc, 128)) return 1;
+  const int num_kb = cdiv(K, BK);
+  DenseProducer<128, true, false> prod{0, 0ull, a_grp, 0};
+  return launch_cfg<128, true, false, DenseProducer<128, true, false>, true, true>(ta, tb, ep, prod, N, M, num_kb, 1, num_kb, s, &tcm);
+}
+
 // a: K-major [M,K] (a_mn=0) or MN-major [K,M] (a_mn=1); b likewise with N.
 int gemm_tf32(const float* a, long long lda, int a_mn, const float* b, long long ldb, int b_mn, Epilogue ep, int M, int N, int K,
               int allow_splitk, cudaStream_t s) {
   if (M <= 0 || N <= 0) return 0;
+  if (a_mn == 0 && b_mn == 1 && !allow_splitk && dgrad_t(ep, N)) return gemm_tf32_t(a, lda, b, ldb, ep, M, N, K, s);
   CUtensorMap ta, tb;
   int BN = (N > 64) ? 128 : 64;
   // Latency-bound GEMMs of the token decoder (a few dozen 128-row tiles, K <= 512): when 128-wide tiles would occupy at most half of the SMs,
@@ -255,6 +286,14 @@ int gemm_tf32(const float* a, long long lda, int a_mn, const float* b, long long
     DenseProducer<bn, am != 0, bm != 0> prod{0, 0ull, a_grp, b_grp};                                             \
     return launch_cfg<bn, am != 0, bm != 0>(ta, tb, ep, prod, M, N, num_kb, splits, kps, s); \
   }
+  // MN-major A (the weight gradients): read into registers by the consumers (rih_set_gemm_rs bit 1)
+#define RIH_TC_CASE_RS(bn)                                                                                        \
+  if ((g_gemm_rs & 2) && BN == bn && a_mn == 1 && b_mn == 1) {                                                    \
+    DenseProducer<bn, true, true> prod{0, 0ull, a_grp, b_grp};                                                    \
+    return launch_cfg<bn, true, true, DenseProducer<bn, true, true>, true>(ta, tb, ep, prod, M, N, num_kb, splits, kps, s); \
+  }
+  RIH_TC_CASE_RS(128) RIH_TC_CASE_RS(64)
+#undef RIH_TC_CASE_RS
   RIH_TC_CASE(128, 0, 0) RIH_TC_CASE(64, 0, 0)
   RIH_TC_CASE(128, 0, 1) RIH_TC_CASE(64, 0, 1)
   RIH_TC_CASE(128, 1, 1) RIH_TC_CASE(64, 1, 1)
@@ -308,10 +347,18 @@ int bgemm_tf32(const BOperand& a, int a_mn, const BOperand& b, int b_mn, const B
   int rc = 1;
   bool matched = false;
 #define RIH_BG_CASE(bn, am, bm)                                                                            \
-  if (BN == bn && a_mn == am && b_mn == bm) {                                                              \
+  if (!matched && BN == bn && a_mn == am && b_mn == bm) {                                                  \
     BatchedProducer<bn, am != 0, bm != 0> prod{H, a.tok, b.tok}; matched = true;                            \
     rc = launch_cfg<bn, am != 0, bm != 0>(ta, tb, ep, prod, M, N, num_kb, B * H, num_kb, s, &tcm);           \
   }
+  // MN-major A (attention dK, dV): read into registers by the consumers (rih_set_gemm_rs bit 1)
+#define RIH_BG_CASE_RS(bn)                                                                                          \
+  if (!matched && (g_gemm_rs & 2) && BN == bn && a_mn == 1 && b_mn == 1) {                                          \
+    BatchedProducer<bn, true, true> prod{H, a.tok, b.tok}; matched = true;                                          \
+    rc = launch_cfg<bn, true, true, BatchedProducer<bn, true, true>, true>(ta, tb, ep, prod, M, N, num_kb, B * H, num_kb, s, &tcm); \
+  }
+  RIH_BG_CASE_RS(128) RIH_BG_CASE_RS(64)
+#undef RIH_BG_CASE_RS
   RIH_BG_CASE(128, 0, 0) RIH_BG_CASE(64, 0, 0) RIH_BG_CASE(128, 0, 1) RIH_BG_CASE(64, 0, 1) RIH_BG_CASE(128, 1, 1) RIH_BG_CASE(64, 1, 1)
 #undef RIH_BG_CASE
   g_scale = keep;
@@ -389,6 +436,11 @@ static int conv_dgrad_s2_direct(const float* dy, const float* w, Epilogue ep, co
   if (make_tmap_nhwc(&tcm, ep.c, g.N, g.H, g.W, g.Cin, ep.ldc, W2, tile_h, tile_n, false, 2)) return 1;
   const int accumulate = ep.mode != 0;
   if (accumulate) { set_error("conv_dgrad_s2_direct: accumulation through an element-strided map is not supported (use the copy-based path)"); return 1; }
+  // transposed form (dgrad_t): the weight map is the A operand, its grouped box holds the BM / 32 chunks of an m tile
+  const bool tr = dgrad_t(ep, g.Cin);
+  CUtensorMap tw;
+  if (tr && (b_grp ? make_tmap_2d_grouped(&tw, w, g.Cout, (long long)g.R * g.S * g.Cin, (long long)g.R * g.S * g.Cin, BM / 32)
+                   : make_tmap_2d(&tw, w, g.Cout, (long long)g.R * g.S * g.Cin, (long long)g.R * g.S * g.Cin, 32, true))) return 1;
   bool zeroed = false;
   for (int ph = 0; ph < 2; ++ph) for (int pw = 0; pw < 2; ++pw) {
     int nr = 0, ns = 0;
@@ -416,10 +468,18 @@ static int conv_dgrad_s2_direct(const float* dy, const float* w, Epilogue ep, co
     e2.M = M; e2.s2_w2 = W2; e2.s2_h2 = H2; e2.s2_ph = ph; e2.s2_pw = pw;
     const int num_kb = nt * cdiv(g.Cout, BK);
     int rc;
-#define RIH_S2_CASE(bn)                                                                                                        \
-    { ConvDgradS2Producer<bn> p{cg, nt, {tap[0], tap[1], tap[2], tap[3]}, {dr[0], dr[1], dr[2], dr[3]}, {ds[0], ds[1], ds[2], ds[3]}, b_grp}; \
-      rc = launch_cfg<bn, false, true>(ta, tb, e2, p, M, g.Cin, num_kb, 1, num_kb, s, &tcm); }
-    if (BN == 128) RIH_S2_CASE(128) else RIH_S2_CASE(64)
+#define RIH_S2_CASE(bn, t)                                                                                                        \
+    ConvDgradS2Producer<bn, t> p{cg, nt, {tap[0], tap[1], tap[2], tap[3]}, {dr[0], dr[1], dr[2], dr[3]}, {ds[0], ds[1], ds[2], ds[3]}, b_grp};
+    if (tr) {
+      RIH_S2_CASE(128, true)
+      rc = launch_cfg<128, true, false, ConvDgradS2Producer<128, true>, true, true>(tw, ta, e2, p, g.Cin, M, num_kb, 1, num_kb, s, &tcm);
+    } else if (BN == 128) {
+      RIH_S2_CASE(128, false)
+      rc = launch_cfg<128, false, true>(ta, tb, e2, p, M, g.Cin, num_kb, 1, num_kb, s, &tcm);
+    } else {
+      RIH_S2_CASE(64, false)
+      rc = launch_cfg<64, false, true>(ta, tb, e2, p, M, g.Cin, num_kb, 1, num_kb, s, &tcm);
+    }
 #undef RIH_S2_CASE
     if (rc) return rc;
   }
@@ -446,6 +506,14 @@ int conv_dgrad_tf32(const float* dy, const float* w, Epilogue ep, const ConvGeom
             : make_tmap_2d(&tb, w, g.Cout, (long long)g.R * g.S * g.Cin, (long long)g.R * g.S * g.Cin, 32, true)) return 1;
   ConvTcGeom cg{g.Cin, g.Cout, g.R, g.S, g.pad, g.H, g.W, g.Ho, g.Wo, tile_h, 0, g.Cin};
   const int num_kb = g.R * g.S * cdiv(g.Cout, BK);
+  if (dgrad_t(ep, g.Cin)) {     // transposed form: A = the weight chunks of an m tile of input channels, B = the dY pixel box
+    CUtensorMap tw, tcm;
+    if (b_grp ? make_tmap_2d_grouped(&tw, w, g.Cout, (long long)g.R * g.S * g.Cin, (long long)g.R * g.S * g.Cin, BM / 32)
+              : make_tmap_2d(&tw, w, g.Cout, (long long)g.R * g.S * g.Cin, (long long)g.R * g.S * g.Cin, 32, true)) return 1;
+    if (make_tmap_2d(&tcm, ep.c, M, g.Cin, ep.ldc, 128)) return 1;
+    ConvDgradProducer<128, true> p{cg, b_grp};
+    return launch_cfg<128, true, false, ConvDgradProducer<128, true>, true, true>(tw, ta, ep, p, g.Cin, M, num_kb, 1, num_kb, s, &tcm);
+  }
   if (BN == 128) { ConvDgradProducer<128> p{cg, b_grp}; return launch_cfg<128, false, true>(ta, tb, ep, p, M, g.Cin, num_kb, 1, num_kb, s); }
   ConvDgradProducer<64> p{cg, b_grp};
   return launch_cfg<64, false, true>(ta, tb, ep, p, M, g.Cin, num_kb, 1, num_kb, s);
@@ -471,7 +539,7 @@ int stem_wgrad_tf32(const float* dy, int lddy, const float* xp, Epilogue ep, int
   int num_kb = P / BK, splits, kps;
   plan_splitk(ep, 64, 224, 128, num_kb, 1, splits, kps, s);
   StemWgradProducer<128> p{Ho, Wo};
-  if (g_gemm_rs) return launch_cfg<128, true, true, StemWgradProducer<128>, true>(ta, tb, ep, p, 64, 224, num_kb, splits, kps, s);
+  if (g_gemm_rs & 1) return launch_cfg<128, true, true, StemWgradProducer<128>, true>(ta, tb, ep, p, 64, 224, num_kb, splits, kps, s);
   return launch_cfg<128, true, true>(ta, tb, ep, p, 64, 224, num_kb, splits, kps, s);
 }
 
@@ -521,11 +589,11 @@ int conv_wgrad_tf32(const float* dy, const float* x, Epilogue ep, const ConvGeom
   }
   if (BN == 128) {
     ConvWgradProducer<128> p{cg, a_grp, wide ? b_grp : 0};
-    if (g_gemm_rs) return launch_cfg<128, true, true, ConvWgradProducer<128>, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap);
+    if (g_gemm_rs & 1) return launch_cfg<128, true, true, ConvWgradProducer<128>, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap);
     return launch_cfg<128, true, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap);
   }
   ConvWgradProducer<64> p{cg, a_grp, 0};
-  if (g_gemm_rs) return launch_cfg<64, true, true, ConvWgradProducer<64>, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap);
+  if (g_gemm_rs & 1) return launch_cfg<64, true, true, ConvWgradProducer<64>, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap);
   return launch_cfg<64, true, true>(ta, tb, ep, p, g.Cout, Ngrid, num_kb, splits, kps, s, cmap);
 }
 

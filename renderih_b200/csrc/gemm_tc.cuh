@@ -197,7 +197,7 @@ struct DenseProducer {
   // single-thread form (fully unrolled).  K-major operands are one box each and stay with lane 0 / lane 1.
   static constexpr bool WIDE_OK = A_MN || B_MN;
   int kbeg;
-  unsigned long long a_policy;   // 0 = no hint
+  unsigned long long a_policy;   // L2 hint of the streamed activation operand (K-major A; K-major B = dY when A is MN-major, the transposed dgrad); 0 = no hint
   // a_grp / b_grp != 0: the MN-major operand comes through a "grouped" rank-3 tensor map {32 columns of a group, k rows, column groups} whose box
   // {32, 32, BM/32 or BN/32} lands in shared memory as the same [group][k row][32] chunks -- ONE TMA operation per operand and k-block
   // instead of one per 32-column chunk (make_tmap_2d_grouped; needs a column count that is a multiple of 32)
@@ -213,7 +213,9 @@ struct DenseProducer {
 #pragma unroll
       for (int c = 0; c < BM / 32; ++c) tma_load_2d(sa + c * (BK * 128), ta, m0 + c * 32, k0, bar);
     }
-    if constexpr (!B_MN) { if (!W || lane == BM / 32) tma_load_2d(sb, tb, k0, n0, bar); }
+    if constexpr (!B_MN) {
+      if (!W || lane == BM / 32) { if (A_MN && a_policy) tma_load_2d_hint(sb, tb, k0, n0, bar, a_policy); else tma_load_2d(sb, tb, k0, n0, bar); }
+    }
     else if (b_grp) { if (!W || lane == BM / 32) tma_load_3d(sb, tb, 0, k0, n0 >> 5, bar); }
     else if constexpr (W) { const int c = lane - BM / 32; if (c >= 0 && c < BN / 32) tma_load_2d(sb + c * (BK * 128), tb, n0 + c * 32, k0, bar); }
     else {
@@ -305,11 +307,14 @@ struct ConvFwdProducer {
   }
 };
 // dgrad (stride 1): A = shifted dY boxes (4-D map over [N,Ho,Wo,Cout]), B = weights as MN-major chunks {32 c, 32 co}
-template <int BN>
+// T (transposed output, dX^T = W^T dY^T): the same boxes with the roles swapped -- ta = the weight map, its chunks go to `sa` (A rows = m0 +
+// 0..127 = input channels, an MN-major A tile that the consumers read into registers), tb = the dY map, its pixel box goes to `sb` (B rows =
+// n0 + 0..127 = pixels, K-major: nothing to transpose).
+template <int BN, bool T = false>
 struct ConvDgradProducer {
   static constexpr bool WIDE_OK = false;     // one or two large boxes per k-block (+ a few weight chunks): issued by lane 0
   ConvTcGeom g;
-  int b_grp;                                 // weights through a grouped rank-3 map: the BN / 32 chunks of a k-block in ONE box (Cin % 32 == 0)
+  int b_grp;                                 // weights through a grouped rank-3 map: the 128 / 32 (T) or BN / 32 chunks of a k-block in ONE box (Cin % 32 == 0)
   __device__ __forceinline__ void set_policy(unsigned long long) {}
   template <bool W>
   __device__ __forceinline__ void load(const CUtensorMap* ta, const CUtensorMap* tb, int kb, int m0, int n0, int z, uint8_t* sa, uint8_t* sb, uint64_t* bar, int lane) const {
@@ -317,18 +322,22 @@ struct ConvDgradProducer {
     const int tap = kb / cpb, co0 = (kb - tap * cpb) * BK;
     const int r = tap / g.S, s = tap - r * g.S;
     const int P = g.H * g.W;
-    const int n = m0 / P, ih0 = (m0 - n * P) / g.W;
-    tma_load_4d(sa, ta, co0, g.pad - s, ih0 + g.pad - r, n, bar);
-    if (b_grp) { tma_load_3d(sb, tb, 0, co0, (tap * g.Cin + n0) >> 5, bar); return; }
+    const int p0 = T ? n0 : m0, c0 = T ? m0 : n0;       // first pixel / first input channel of the tile
+    const int n = p0 / P, ih0 = (p0 - n * P) / g.W;
+    tma_load_4d(T ? sb : sa, T ? tb : ta, co0, g.pad - s, ih0 + g.pad - r, n, bar);
+    uint8_t* sw = T ? sa : sb;
+    const CUtensorMap* tw = T ? ta : tb;
+    if (b_grp) { tma_load_3d(sw, tw, 0, co0, (tap * g.Cin + c0) >> 5, bar); return; }
 #pragma unroll
-    for (int c = 0; c < BN / 32; ++c) tma_load_2d(sb + c * (BK * 128), tb, tap * g.Cin + n0 + c * 32, co0, bar);
+    for (int c = 0; c < (T ? BM : BN) / 32; ++c) tma_load_2d(sw + c * (BK * 128), tw, tap * g.Cin + c0 + c * 32, co0, bar);
   }
 };
 // dgrad of a stride-2 convolution, one PARITY CLASS of input pixels (ih, iw) = (2 i + ph, 2 j + pw): only the taps r = ph + pad (mod 2),
 // s = pw + pad (mod 2) reach those pixels, from output pixel (i + dr, j + ds) with dr = (ph + pad - r) / 2.  Each class is a dense
 // stride-1 problem over the half-resolution grid: A = dY boxes shifted by (dr, ds), B = that tap's weights (MN-major chunks), K = ntaps * Cout;
 // the four classes together do a quarter of the multiply-adds of "zero-insert dY, then a stride-1 dgrad" and need no dilated copy.
-template <int BN>
+// T: transposed output, operands swapped as in ConvDgradProducer.
+template <int BN, bool T = false>
 struct ConvDgradS2Producer {
   static constexpr bool WIDE_OK = false;     // one or two large boxes per k-block (+ a few weight chunks): issued by lane 0
   ConvTcGeom g;            // H, W = half-resolution grid of the class (= Ho, Wo of the convolution); tile_h as usual
@@ -341,11 +350,14 @@ struct ConvDgradS2Producer {
     const int cpb = (g.Cout + BK - 1) / BK;
     const int ti = kb / cpb, co0 = (kb - ti * cpb) * BK;
     const int P = g.H * g.W;
-    const int n = m0 / P, i0 = (m0 - n * P) / g.W;
-    tma_load_4d(sa, ta, co0, ds[ti], i0 + dr[ti], n, bar);
-    if (b_grp) { tma_load_3d(sb, tb, 0, co0, (tap[ti] * g.Cin + n0) >> 5, bar); return; }
+    const int p0 = T ? n0 : m0, c0 = T ? m0 : n0;
+    const int n = p0 / P, i0 = (p0 - n * P) / g.W;
+    tma_load_4d(T ? sb : sa, T ? tb : ta, co0, ds[ti], i0 + dr[ti], n, bar);
+    uint8_t* sw = T ? sa : sb;
+    const CUtensorMap* tw = T ? ta : tb;
+    if (b_grp) { tma_load_3d(sw, tw, 0, co0, (tap[ti] * g.Cin + c0) >> 5, bar); return; }
 #pragma unroll
-    for (int c = 0; c < BN / 32; ++c) tma_load_2d(sb + c * (BK * 128), tb, tap[ti] * g.Cin + n0 + c * 32, co0, bar);
+    for (int c = 0; c < (T ? BM : BN) / 32; ++c) tma_load_2d(sw + c * (BK * 128), tw, tap[ti] * g.Cin + c0 + c * 32, co0, bar);
   }
 };
 // wgrad: A = dY as MN-major chunks {32 co, 32 pixels}, B = shifted input boxes of 32 pixels as MN-major chunks {32 c, 32 pixels}.
@@ -638,10 +650,17 @@ template <int NSPLIT> __device__ __forceinline__ void split_frag(const uint32_t 
 // warpgroup handles B alone and is dropped when B needs nothing.
 // tma_epi != 0: the epilogue writes 32-column chunks with TMA stores (cp.reduce.async.bulk ... .add for accumulate / split-K), fully coalesced
 // and clipped at the tensor edge by the hardware.
+// OUT_T (transposed output; A_RS, K-major B, BN == 128): the kernel computes D^T of the output it stores.  The input gradients run this way,
+// dX^T[channels, pixels] = W^T dY^T, so that the weights are the MN-major A operand the consumers read into registers and dY a K-major B
+// operand -- no operand is transposed in shared memory.  The accumulator is staged transposed (BM / 32 chunks of [BN rows x 128 B], one per
+// 32 output columns) and stored with tmap_c / ep over the [pixels x channels] output; only ep.scale and store / accumulate (mode 0 / 1) apply.
+// Tile order: the m tiles (channels) of one n tile (pixels) run on neighbouring CTAs, so a dY tile is fetched from HBM once and then hit in L2.
+// This numbers every output tile exactly as the untransposed product with 128-wide tiles does, so the k-block rotation (rih_set_k_rotation),
+// which starts a tile's k loop at (tile index) % (k-blocks), and the reverse traversal give both forms the same k order per output element.
 template <bool A_MN, bool B_MN, int NSPLIT, bool A_RS = false> __host__ __device__ constexpr bool has_prep() { return (A_MN && !A_RS) || B_MN || NSPLIT >= 2; }
 template <bool A_MN, bool B_MN, int NSPLIT, bool A_RS = false> __host__ __device__ constexpr int persistent_threads() { return (has_prep<A_MN, B_MN, NSPLIT, A_RS>() ? 4 : 3) * 128; }
 
-template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT, bool A_RS = false>
+template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT, bool A_RS = false, bool OUT_T = false>
 __global__ void __launch_bounds__(persistent_threads<A_MN, B_MN, NSPLIT, A_RS>(), 1)
 gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_c,
                           Epilogue ep, Producer prod, int num_kb_total, int kb_per_split, int tiles_m, int tiles_n, int splits, int tma_epi) {
@@ -649,6 +668,7 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
   constexpr int A_BYTES = BM * 128, B_BYTES = BN * 128, AB_BYTES = A_BYTES + B_BYTES;
   constexpr int STAGE_BYTES = stage_bytes<BN, NSPLIT>();
   static_assert(!A_RS || A_MN, "the register-A main loop reads MN-major A tiles");
+  static_assert(!OUT_T || (A_RS && !B_MN && BN == BM), "transposed output: register-A main loop, K-major B, square 128 x 128 tiles");
   constexpr bool PREP = has_prep<A_MN, B_MN, NSPLIT, A_RS>();
   constexpr int CONS_WARP0 = PREP ? 8 : 4;
   constexpr int EPI_WG = 2;
@@ -679,10 +699,18 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
   const bool batched = ep.batch_heads != 0;
   auto tile_coords = [&](int t, int& m0, int& n0, int& kb_beg, int& nkb, int& z) {
     if (ep.reverse) t = total_tiles - 1 - t;          // serpentine traversal across consecutive kernels (rih_set_traversal)
-    const int ni = t % tiles_n;
-    const int r = t / tiles_n;
-    const int mi = r % tiles_m;
-    z = r / tiles_m;
+    int mi, ni;
+    if constexpr (OUT_T) {                            // the output's columns (m tiles) fastest, as for the untransposed product
+      mi = t % tiles_m;
+      const int r = t / tiles_m;
+      ni = r % tiles_n;
+      z = r / tiles_n;
+    } else {
+      ni = t % tiles_n;
+      const int r = t / tiles_n;
+      mi = r % tiles_m;
+      z = r / tiles_m;
+    }
     m0 = mi * BM; n0 = ni * BN;
     kb_beg = batched ? 0 : z * kb_per_split;
     nkb = batched ? num_kb_total : min(num_kb_total - kb_beg, kb_per_split);
@@ -746,7 +774,8 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
     const int rr = q * 32 + lane;                   // epilogue row of this thread inside the tile
     const bool elected = (threadIdx.x == (CONS_WARP0 + 4 * wg) * 32);
     const unsigned long long dseed = ep.thresh ? (*ep.seed_ptr + ep.site * 0xD1B54A32D192ED03ull) : 0ull;
-    constexpr int NCHUNK = BN / 32;
+    constexpr int NCHUNK = (OUT_T ? BM : BN) / 32;     // 32-column chunks of the stored tile
+    constexpr int CHUNK_ROWS = OUT_T ? BN : BM;       // rows of the stored tile
     // fused BatchNorm statistics: per-thread fp64 accumulators (lane = column of a chunk, warp = row quarter), carried ACROSS the tiles of this
     // persistent CTA and flushed with one atomic pair per column when the CTA moves to another column block / at the end: flushing per tile
     // put ~10^6 fp64 atomics per convolution onto 2 N addresses, serialised in the L2.
@@ -765,8 +794,9 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
         }
       }
     };
-    const bool use_res = tma_epi && ep.res != nullptr && !batched && !ep.nv_pad && (ep.opt & 1);
-    const bool use_cv = tma_epi && !batched && !ep.nv_pad && (ep.bias != nullptr || ep.col_scale != nullptr) && (ep.opt & 2);
+    const bool do_stats = !OUT_T && ep.stats != nullptr;
+    const bool use_res = !OUT_T && tma_epi && ep.res != nullptr && !batched && !ep.nv_pad && (ep.opt & 1);
+    const bool use_cv = !OUT_T && tma_epi && !batched && !ep.nv_pad && (ep.bias != nullptr || ep.col_scale != nullptr) && (ep.opt & 2);
     float4 rcur[8], rnext[8];
     int cv_n0 = -1;
     uint32_t it = 0;
@@ -804,9 +834,13 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
             wgmma_fence();
             const uint64_t bd = make_wgmma_desc(sb + ks * 32);
             wgmma_tf32_rs<BN>(acc, ahi[ks & 1], bd);
-            if constexpr (NSPLIT == 3) {
+            if constexpr (NSPLIT == 3 && !OUT_T) {
               wgmma_tf32_rs<BN>(acc, alo[ks & 1], bd);                              // lo(A) * hi(B)
               wgmma_tf32_rs<BN>(acc, ahi[ks & 1], bd + (uint64_t)(AB_BYTES >> 4));  // hi(A) * lo(B)
+            } else if constexpr (NSPLIT == 3) {
+              // the untransposed product's order: lo of the output's row operand (here B) times hi of its column operand first
+              wgmma_tf32_rs<BN>(acc, ahi[ks & 1], bd + (uint64_t)(AB_BYTES >> 4));  // hi(A) * lo(B)
+              wgmma_tf32_rs<BN>(acc, alo[ks & 1], bd);                              // lo(A) * hi(B)
             }
             wgmma_commit();
           }
@@ -844,7 +878,27 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
       if (use_res) load_res_chunk(rcur, ep, m, n0 + wg * 32);
       if (elected && tma_epi) tma_store_wait_read<0>();
       cons_bar_sync();
-      {
+      if constexpr (OUT_T) {
+        // Transposed: element (m, n) of the tile goes to chunk m / 32, row n, column m % 32.  Thread (g, t) = (lane / 4, lane % 4) stores
+        // 32-bit words: for register 4 j + 2 h + i, m = r0 + 8 h and n = 8 j + 2 t + i, at unit ((m % 32) >> 2) ^ (n & 7) = ((m' >> 2) ^ (2 t + i))
+        // of row n, word m & 3.  Per store instruction (j, h, i fixed) the warp's m' >> 2 = u0 + (g >> 2) with u0 even, so the unit is
+        // (u0 ^ 2 t) | ((g >> 2) ^ i): 4 values of t x 2 of g >> 2 = 8 distinct units, times 4 words (g & 3) = all 32 banks -- conflict-free
+        // (the row adds a multiple of 128 B and does not move the bank).
+        const int r0 = wg * 64 + q * 16 + (lane >> 2);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int mm = r0 + 8 * h;
+          uint8_t* chunk = accbuf + (mm >> 5) * (BN * 128);
+          const int un = (mm & 31) >> 2, wo = (mm & 3) << 2;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const int nn = 8 * j + 2 * (lane & 3) + i;
+              *reinterpret_cast<float*>(chunk + nn * 128 + ((un ^ (nn & 7)) << 4) + wo) = acc[4 * j + 2 * h + i];
+            }
+        }
+      } else {
         // wgmma D fragment: register 4 j + {0, 1} = row (warp q) * 16 + lane / 4, columns 8 j + 2 (lane % 4) + {0, 1}; + {2, 3} = 8 rows below
         const int r0 = wg * 64 + q * 16 + (lane >> 2);
 #pragma unroll
@@ -870,7 +924,7 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
         cv_n0 = n0;
       }
       cons_bar_sync();
-      if (ep.stats && n0 != acc_n0) { flush_stats(); acc_n0 = n0; }
+      if (do_stats && n0 != acc_n0) { flush_stats(); acc_n0 = n0; }
 
       // ---- epilogue of this warpgroup's chunks: thread = row rr, 32 columns
 #pragma unroll 1
@@ -882,14 +936,16 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
           }
           if (c + EPI_WG < NCHUNK) load_res_chunk(rnext, ep, m, n0 + (c + EPI_WG) * 32);
         }
-        uint8_t* buf = accbuf + c * (BM * 128);
+        uint8_t* buf = accbuf + c * (CHUNK_ROWS * 128);
         float v[32];
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float4 x = *reinterpret_cast<const float4*>(buf + rr * 128 + ((j ^ (rr & 7)) << 4));
           v[4 * j] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w;
         }
-        const int nb = n0 + c * 32;
+        const int nb = (OUT_T ? m0 : n0) + c * 32;       // first output column of the chunk
+        const int row0 = OUT_T ? n0 : m0;                // first output row of the tile
+        if (OUT_T && nb >= ep.N) continue;               // rows of A beyond the output's columns (e.g. the next tap's weights): never stored
         int sc0 = nb, sc1 = 0;
         if (ep.nv_pad) {               // virtual wgrad column -> (channel, tap); chunks wholly beyond Cin are skipped (warp-uniform)
           sc1 = nb / ep.nv_pad; sc0 = nb - sc1 * ep.nv_pad;
@@ -911,17 +967,17 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
               else tma_store_4d(&tmap_c, buf, nb, z % hh, m0, z / hh);                        // head slice of a token matrix
             } else if (ep.s2_w2) {           // stride-2 dgrad parity class: rows (n, i, j) -> input pixels (2 i + ph, 2 j + pw), element-strided 4-D map
               const int P2 = ep.s2_h2 * ep.s2_w2;
-              const int n_ = m0 / P2, i0 = (m0 - n_ * P2) / ep.s2_w2;
+              const int n_ = row0 / P2, i0 = (row0 - n_ * P2) / ep.s2_w2;
               if (ep.mode == 0) tma_store_4d(&tmap_c, buf, nb, ep.s2_pw, 2 * i0 + ep.s2_ph, n_);
               else tma_reduce_add_4d(&tmap_c, buf, nb, ep.s2_pw, 2 * i0 + ep.s2_ph, n_);
             } else if (ep.nv_pad) {
               if (ep.mode == 0) tma_store_3d(&tmap_c, buf, sc0, sc1, m0);
               else tma_reduce_add_3d(&tmap_c, buf, sc0, sc1, m0);
-            } else if (ep.mode == 0) tma_store_2d(&tmap_c, buf, nb, m0);
-            else tma_reduce_add_2d(&tmap_c, buf, nb, m0);
+            } else if (ep.mode == 0) tma_store_2d(&tmap_c, buf, nb, row0);
+            else tma_reduce_add_2d(&tmap_c, buf, nb, row0);
             tma_store_commit();
           }
-          if (ep.stats) {
+          if (do_stats) {
             // fused BatchNorm statistics: column sums / sums of squares of the chunk over this warp's 32 rows.  Each lane holds one ROW
             // (32 columns) in registers: a halving butterfly over the lanes (16 + 8 + 4 + 2 + 1 = 31 exchanges per quantity) leaves lane l with
             // the totals of column l.  Then one fp64 atomic pair per column per warp when the column block changes.
@@ -953,7 +1009,7 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
         }
       }
     }
-    if (ep.stats) flush_stats();
+    if (do_stats) flush_stats();
     if (elected && tma_epi) tma_store_wait<0>();
   }
 }
