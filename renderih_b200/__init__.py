@@ -26,6 +26,10 @@ Public API mirrors the reference modules it replaces:
     GeOptimizer                         <-  pose_data_optimize/hocontact/postprocess/geo_optimizer_both_batch.py:22-930 (ge_optimizer.py:
                                             the two-hand pose optimiser, set_opt_val / optimize, one CUDA graph per iteration with
                                             device-side Adam and ReduceLROnPlateau)
+    hand_collision_count, filter_collision_data  <-  pose_data_optimize/collision/CollisionFilter.py:9-127, CollisionCheck.py
+                                            (collision.py: per-frame count of intersecting face pairs between the two hand meshes)
+    ValidJudger, get_valid_rate         <-  pose_data_optimize/Ver2Code/ValidJudge/ValidJudger.py, GetValidRate.py (valid_judge.py:
+                                            the joint-limit validity rate of both hands)
 """
 from . import _build
 
@@ -69,6 +73,12 @@ def __getattr__(name):
     if name == 'GeOptimizer':
         from . import ge_optimizer
         return ge_optimizer.GeOptimizer
+    if name in ('hand_collision_count', 'filter_collision_data'):
+        from . import collision
+        return getattr(collision, name)
+    if name in ('ValidJudger', 'get_valid_rate'):
+        from . import valid_judge
+        return getattr(valid_judge, name)
     if name in ('load_cfg', 'get_cfg_defaults'):
         from . import config
         return getattr(config, name)

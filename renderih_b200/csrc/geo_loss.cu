@@ -12,6 +12,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "hand_pose.cuh"
 using namespace rih;
 
 namespace {
@@ -33,12 +34,6 @@ struct GeoConsts {
   const float* conv;      // [2,15,18] per hand and joint 1..15: P (row-major 3x3) then C
 };
 
-// hand_pose_ergonomics_loss limits per ergonomics index t (joint t + 1), geo_loss.py:399-414
-__constant__ float c_bend_lo[NJ] = {-25, -4, -8, -25, -7, -8, -22, -8, -8, -25, -10, -8, -20, -35, -10};
-__constant__ float c_bend_hi[NJ] = {70, 110, 90, 80, 100, 90, 70, 90, 90, 70, 100, 90, 40, 50, 100};
-__constant__ float c_spl_lo[NJ] = {-25, 0, 0, -15, 0, 0, -20, 0, 0, -25, 0, 0, -30, 0, 0};   // used where t % 3 == 0
-__constant__ float c_spl_hi[NJ] = {15, 0, 0, 15, 0, 0, 30, 0, 0, 15, 0, 0, 30, 0, 0};
-
 __device__ __forceinline__ float block_sum(float v, float* s_red, int tid) {
   v = warp_sum(v);
   __syncthreads();
@@ -57,20 +52,6 @@ __device__ __forceinline__ void anchor_pos(const float* vb, const int* f, const 
     const float b1 = __fsub_rn(vb[f[1] * 3 + c], o), b2 = __fsub_rn(vb[f[2] * 3 + c], o);
     out[c] = __fadd_rn(__fadd_rn(__fmul_rn(w[0], b1), __fmul_rn(w[1], b2)), o);
   }
-}
-
-// quatutils.py:191-216: entries of the rotation matrix over |q|^2
-__device__ __forceinline__ void quat_to_R(float w, float x, float y, float z, float* R) {
-  const float ww = w * w, wx = w * x, wy = w * y, wz = w * z, xx = x * x, xy = x * y, xz = x * z, yy = y * y, yz = y * z, zz = z * z;
-  const float n = ww + xx + yy + zz;
-  R[0] = (ww + xx - yy - zz) / n; R[1] = 2.f * (xy - wz) / n;       R[2] = 2.f * (wy + xz) / n;
-  R[3] = 2.f * (wz + xy) / n;     R[4] = (ww - xx + yy - zz) / n;   R[5] = 2.f * (yz - wx) / n;
-  R[6] = 2.f * (xz - wy) / n;     R[7] = 2.f * (wx + yz) / n;       R[8] = (ww - xx - yy + zz) / n;
-}
-
-__device__ __forceinline__ void mat3_mul(const float* A, const float* B, float* C) {
-  for (int r = 0; r < 3; ++r)
-    for (int c = 0; c < 3; ++c) C[r * 3 + c] = A[r * 3] * B[c] + A[r * 3 + 1] * B[3 + c] + A[r * 3 + 2] * B[6 + c];
 }
 
 // F.normalize(q, eps=1e-12) (quatutils.py:7-30), the left hand's (w, x, -y, -z) (HandPoseConverter.py:220-222), R, then M = P R C.
