@@ -278,97 +278,61 @@ class resnet_mid(nn.Module):
 
 
 # ============================================================================ two-hand concurrency
-class HandStreams:
-    """The left- and right-hand sub-graphs of a DualGraph level are independent until `inter_attn` mixes them, and each of their
-    kernels (4032 ... 16128 token rows) fills well under half of the 132 SMs of an H100.  Running them on two side streams lets the GPU overlap
-    them; under CUDA-graph capture the fork/join becomes two parallel branches of the graph.  autograd replays each backward node on
-    its forward stream, so the backward pass is two-stream as well.  `RIH_HAND_STREAMS=0` disables it (single stream)."""
-    _cache = {}
+# The forward pass overlaps independent work on five side streams per device; under CUDA-graph capture each fork / join becomes a pair
+# of parallel graph branches, and autograd replays every backward node on its forward stream, so the backward pass overlaps the same way.
+#   left, right   the two hands' sub-graphs of a DualGraph level, independent until `inter_attn` mixes them.  Each of their kernels
+#                 (4032 ... 16128 token rows) fills well under half of the H100's 132 SMs.  High priority: the latency-bound hand
+#                 branches are scheduled ahead of concurrent convolution work.
+#   grid0, grid1  the image-grid encoders of a DualGraph level, which depend only on the image feature map.
+#   aux           the convolution side of HandNET_GCN behind the trunk (heat-map / dense-pose stages, mid levels, aux heads).
+_SIDE_STREAMS = {}
 
-    @classmethod
-    def get(cls, device):
-        import os
-        if os.environ.get('RIH_HAND_STREAMS', '1') == '0':
-            return None
-        key = (device.type, device.index)
-        if key not in cls._cache:
-            prio = int(os.environ.get('RIH_HAND_PRIORITY', '-1'))      # -1: the (latency-bound) hand branches are scheduled ahead of concurrent convolution work
-            cls._cache[key] = (torch.cuda.Stream(device=device, priority=prio), torch.cuda.Stream(device=device, priority=prio))
-            ctas = int(os.environ.get('RIH_HAND_CTAS', '0'))             # > 0: cap the persistent GEMM grids of each hand branch (several tiles per CTA amortise the
-            if ctas > 0:                                               # per-CTA prologue and leave SMs to the other branches); 0 = uncapped
-                from ._lib import call
-                for st in cls._cache[key]:
-                    call('rih_set_stream_cta_limit', st.cuda_stream, ctas)
+
+def _side_stream(device, role):
+    key = (device.type, device.index, role)
+    st = _SIDE_STREAMS.get(key)
+    if st is None:
+        st = _SIDE_STREAMS[key] = torch.cuda.Stream(device=device, priority=-1 if role in ('left', 'right') else 0)
+        if role == 'aux':
+            # cap the persistent grid of the tensor-core GEMMs / convolutions launched on it, leaving the other SMs to the token decoder
+            # while the convolution pipeline runs.  72 was chosen on a 148-SM GPU and has not been tuned on the H100 (132 SMs).
+            from ._lib import call
+            call('rih_set_stream_cta_limit', st.cuda_stream, 72)
+        elif role == 'left':
             try:      # parameters shared by both hands accumulate gradients from two streams by design; silence torch's advisory
                 torch.autograd.graph.set_warn_on_accumulate_grad_stream_mismatch(False)
             except Exception:
                 pass
-        return cls._cache[key]
+    return st
 
 
-def run_hands(device, fn_left, fn_right):
-    """(fn_left(), fn_right()) -- concurrently on two side streams when enabled.  Every tensor a branch returns is registered with the
-    caching allocator as used by the joining stream (it was allocated on the side stream's pool)."""
-    st = HandStreams.get(device)
-    if st is None:
-        return fn_left(), fn_right()
-    main = torch.cuda.current_stream(device)
-    outs = []
-    for s, fn in zip(st, (fn_left, fn_right)):
-        s.wait_stream(main)
-        ops.note_stream(s)
-        with torch.cuda.stream(s):
-            outs.append(fn())
-    for s, o in zip(st, outs):
-        main.wait_stream(s)
-        for t in (o if isinstance(o, (tuple, list)) else (o,)):
-            if torch.is_tensor(t):
-                t.record_stream(main)
-    return outs[0], outs[1]
-
-
-class GridStreams:
-    """Two more side streams for work that depends only on the image feature maps (`RIH_GRID_STREAMS=0` disables them)."""
-    _cache = {}
-
-    @classmethod
-    def get(cls, device):
-        import os
-        if os.environ.get('RIH_GRID_STREAMS', '1') == '0' or HandStreams.get(device) is None:
-            return None
-        key = (device.type, device.index)
-        if key not in cls._cache:
-            cls._cache[key] = (torch.cuda.Stream(device=device), torch.cuda.Stream(device=device))
-        return cls._cache[key]
-
-
-def start_side(device, which, fn):
-    """Launch fn() on grid stream `which`, forked off the current stream, WITHOUT joining.  -> handle for `join_side` (the value itself when the
-    side streams are disabled: then fn is deferred to the join point, i.e. the sequential order)."""
-    st = GridStreams.get(device)
-    if st is None:
-        return ['deferred', fn]
-    s = st[which]
+def fork(device, role, fn):
+    """Run fn() on side stream `role`, forked off the current stream, without joining.  -> handle for `join`."""
+    s = _side_stream(device, role)
     s.wait_stream(torch.cuda.current_stream(device))
     ops.note_stream(s)
     with torch.cuda.stream(s):
         out = fn()
         ev = torch.cuda.Event()
         ev.record(s)
-    return ('started', out, ev)
+    return out, ev
 
 
-def join_side(handle):
-    """Make the CURRENT stream wait for a `start_side` branch and hand over its result."""
-    if handle[0] == 'deferred':
-        if len(handle) == 2:                 # evaluate once, hand the same result to every joiner
-            handle += (handle[1](),)
-        return handle[2]
-    _, out, ev = handle
+def join(handle):
+    """Make the current stream wait for a `fork` branch and hand over its result.  Every tensor in it is registered with the caching
+    allocator as used by the joining stream (it was allocated on the side stream's pool)."""
+    out, ev = handle
     cur = torch.cuda.current_stream()
     cur.wait_event(ev)
     _record_stream_tree(out, cur)
     return out
+
+
+def run_hands(device, fn_left, fn_right):
+    """(fn_left(), fn_right()) run concurrently on the two hand streams."""
+    left = fork(device, 'left', fn_left)
+    right = fork(device, 'right', fn_right)
+    return join(left), join(right)
 
 
 # ============================================================================ decoder blocks (models/model_attn/*.py)
@@ -572,7 +536,7 @@ class img_ex(nn.Module):
         self.G = grid_size * grid_size
 
     def forward(self, img, verts_f, B, V, grid=None):
-        """grid: the image-grid tokens when they were already produced on another stream (`start_grid`)."""
+        """grid: the image-grid tokens when they were already produced on another stream (`fork`)."""
         if grid is None:
             grid = self.encoder(img, B)
         return self.attn(verts_f, grid, B, V, self.G)
@@ -655,11 +619,11 @@ class DualGraphLayer(nn.Module):
         V = self.verts_num
         # the image-grid tokens (patch GEMM + position embedding + a 64-token SelfAttn, ~14 launches per hand) depend only on the feature map:
         # they start on their own streams now and run beside the 28-launch graph-convolution chains of the two hands
-        gp = start_side(Lf.device, 0, lambda: self.img_ex_left.encoder.patches(img_f, B))      # one patch matrix per level, shared by both hands
-        gl = start_side(Lf.device, 0, lambda: self.img_ex_left.encoder(img_f, B, patches=join_side(gp)))
-        gr = start_side(Lf.device, 1, lambda: self.img_ex_right.encoder(img_f, B, patches=join_side(gp)))
-        Lf, Rf = run_hands(Lf.device, lambda: self.img_ex_left(img_f, self.graph_left(Lf, B, V), B, V, grid=join_side(gl)),
-                           lambda: self.img_ex_right(img_f, self.graph_right(Rf, B, V), B, V, grid=join_side(gr)))
+        gp = fork(Lf.device, 'grid0', lambda: self.img_ex_left.encoder.patches(img_f, B))      # one patch matrix per level, shared by both hands
+        gl = fork(Lf.device, 'grid0', lambda: self.img_ex_left.encoder(img_f, B, patches=join(gp)))
+        gr = fork(Lf.device, 'grid1', lambda: self.img_ex_right.encoder(img_f, B, patches=join(gp)))
+        Lf, Rf = run_hands(Lf.device, lambda: self.img_ex_left(img_f, self.graph_left(Lf, B, V), B, V, grid=join(gl)),
+                           lambda: self.img_ex_right(img_f, self.graph_right(Rf, B, V), B, V, grid=join(gr)))
         return self.attn(Lf, Rf, B, V)
 
 
@@ -828,9 +792,8 @@ class HandNET_GCN(nn.Module):
         N = img.shape[0]
         # inference: ONE launch folds every BatchNorm of the network into (scale, shift) vectors for the convolution epilogues
         fold_done = (not (self.encoder.training and self.mid_model.training)) and ops.bn_fold_refresh(self)
-        aux = AuxStream.get(img.device) if (type(self.encoder) is ResNetSimple and self.encoder.aux_heads and type(self.mid_model) is resnet_mid) else None
-        if aux is not None:
-            result, paramsDict, handDictList, otherInfo, hms, mask, dp = self._forward_pipelined(img, N, aux, fold_done)
+        if type(self.encoder) is ResNetSimple and self.encoder.aux_heads and type(self.mid_model) is resnet_mid:
+            result, paramsDict, handDictList, otherInfo, hms, mask, dp = self._forward_pipelined(img, N, fold_done)
         else:
             hms, mask, dp, img_fmaps, hms_fmaps, dp_fmaps = self.encoder(img)
             global_feature, fmaps = self.mid_model(img_fmaps, hms_fmaps, dp_fmaps, N)
@@ -844,79 +807,31 @@ class HandNET_GCN(nn.Module):
         return result, paramsDict, handDictList, otherInfo
 
 
-    def _forward_pipelined(self, img, N, aux, fold_done=False):
+    def _forward_pipelined(self, img, N, fold_done=False):
         """Same arithmetic as encoder -> mid_model -> decoder, issued as two concurrent pipelines: everything behind the trunk on the
         convolution side (heat-map / dense-pose decoder stages at 8, 16, 32, 64 px, the mid 1x1 convs, the aux heads) runs on the aux stream
         and publishes each mid level with an event; the token decoder (main + hand streams) waits for level i only when DualGraph layer i
         starts.  DualGraph layer 1 overlaps the 16 px stage, layer 2 the 32 px stage, layer 3 the 64 px stage + heads, which nothing in the
         decoder reads.  autograd replays every node on its forward stream, so the backward pass is pipelined the same way."""
         enc, mid = self.encoder, self.mid_model
-        dev = img.device
         img_fmaps = enc.trunk(img, fold_done)
         x1, H1 = img_fmaps[0]
         global_feature = ops.global_avgpool(x1, N, H1 * H1)
-        main = torch.cuda.current_stream(dev)
-        aux.wait_stream(main)
-        ops.note_stream(aux)
-        fmaps, events = [], []
-        with torch.cuda.stream(aux):
+        fmaps = _StreamedFmaps()
+
+        def conv_side():
             xh, xd, H = x1, x1, H1
             for i in range(len(mid.convs)):
                 xh, Hn = enc.hms_decoder.stage(i, xh, N, H)
                 xd, _ = enc.dp_decoder.stage(i, xd, N, H)
                 H = Hn
-                fmaps.append(mid.level(i, img_fmaps, (xh, H), (xd, H), N))
-                ev = torch.cuda.Event()
-                ev.record(aux)
-                events.append(ev)
+                fmaps.publish(mid.level(i, img_fmaps, (xh, H), (xd, H), N))
             hms, mask, dp = enc.aux_outputs(enc.hms_decoder.head(xh, N, H), enc.dp_decoder.head(xd, N, H), N, H)
-        dec = AuxStream.decoder_stream(dev)
-        if dec is None:
-            out = self.decoder(global_feature, _StreamedFmaps(fmaps, events))
-        else:       # the token decoder's joint (two-hand) parts on a high-priority stream as well, like its hand branches
-            dec.wait_stream(main)
-            with torch.cuda.stream(dec):
-                out = self.decoder(global_feature, _StreamedFmaps(fmaps, events))
-            main.wait_stream(dec)
-            _record_stream_tree(out, main)
-            global_feature.record_stream(dec)
-        main.wait_stream(aux)
-        for t in (hms, mask, dp) + tuple(f[0] for f in fmaps):
-            t.record_stream(main)
+            return hms, mask, dp, list(fmaps)
+        side = fork(img.device, 'aux', conv_side)
+        out = self.decoder(global_feature, fmaps)
+        hms, mask, dp, _ = join(side)
         return out + (hms, mask, dp)
-
-
-class AuxStream:
-    """Side stream of HandNET_GCN._forward_pipelined; `RIH_AUX_STREAM=0` (or `RIH_HAND_STREAMS=0`) selects the sequential forward.
-    `RIH_AUX_CTAS` caps the persistent grid of the tensor-core GEMMs / convolutions launched on it (0 = all SMs)."""
-    _cache = {}
-
-    @classmethod
-    def get(cls, device):
-        import os
-        if os.environ.get('RIH_AUX_STREAM', '1') == '0' or HandStreams.get(device) is None:
-            return None
-        key = (device.type, device.index)
-        if key not in cls._cache:
-            cls._cache[key] = torch.cuda.Stream(device=device)
-            ctas = int(os.environ.get('RIH_AUX_CTAS', '72'))        # about half of the SMs; not tuned on the H100 (RIH_AUX_CTAS=0: uncapped)
-            if ctas > 0:        # leave 148 - ctas SMs to the token decoder while the convolution pipeline runs
-                from ._lib import call
-                call('rih_set_stream_cta_limit', cls._cache[key].cuda_stream, ctas)
-        return cls._cache[key]
-
-    _dec = {}
-
-    @classmethod
-    def decoder_stream(cls, device):
-        import os
-        prio = int(os.environ.get('RIH_DEC_PRIORITY', '0'))
-        if prio == 0:
-            return None
-        key = (device.type, device.index)
-        if key not in cls._dec:
-            cls._dec[key] = torch.cuda.Stream(device=device, priority=prio)
-        return cls._dec[key]
 
 
 def _record_stream_tree(obj, stream):
@@ -934,9 +849,16 @@ def _record_stream_tree(obj, stream):
 class _StreamedFmaps(list):
     """List of (feature map, H) pairs produced on another stream: the consuming stream waits for a level's event when that level is read."""
 
-    def __init__(self, fmaps, events):
+    def __init__(self, fmaps=(), events=()):
         super().__init__(fmaps)
         self.events = list(events)
+
+    def publish(self, level):
+        """Append a (feature map, H) level and record an event on the current (producing) stream."""
+        ev = torch.cuda.Event()
+        ev.record()
+        self.append(level)
+        self.events.append(ev)
 
     def __getitem__(self, i):
         if isinstance(i, slice):

@@ -21,7 +21,7 @@ from . import ops
 from .assets import default_asset_root, load_mano_dict, load_model_assets
 from .config import load_cfg
 from .manolayer import ManoLayer
-from .model import AuxStream, MLP_GraphBlock, ResNetSimple, _StreamedFmaps, _cl, _conv_relu_bn, decoder as _decoder_base
+from .model import MLP_GraphBlock, ResNetSimple, _StreamedFmaps, _cl, _conv_relu_bn, decoder as _decoder_base, fork, join
 
 
 class resnet_mid(nn.Module):
@@ -228,27 +228,22 @@ class HandNET_GCN(nn.Module):
             ops.seed_state.advance(img.device)
         N = img.shape[0]
         img_fmaps = self.encoder(img)
-        aux = AuxStream.get(img.device) if (type(self.mid_model) is resnet_mid and os.environ.get('RIH_AUX_STREAM_GRAPH', '1') != '0') else None
-        if aux is None:
+        if type(self.mid_model) is not resnet_mid:
             global_feature, fmaps = self.mid_model(img_fmaps, N)
             return self.decoder(global_feature, fmaps)
         # same pipelining as models.model.HandNET_GCN._forward_pipelined: the four mid 1x1 conv + BN levels run on the aux stream, each level's
         # event gates the DualGraph layer that reads it (the 64 px level feeds nothing in the decoder and overlaps all of it)
         x1, H1 = img_fmaps[0]
         global_feature = ops.global_avgpool(x1, N, H1 * H1)
-        main = torch.cuda.current_stream(img.device)
-        aux.wait_stream(main)
-        fmaps, events = [], []
-        with torch.cuda.stream(aux):
+        fmaps = _StreamedFmaps()
+
+        def mid_levels():
             for i in range(len(self.mid_model.convs)):
-                fmaps.append(self.mid_model.level(i, img_fmaps, N))
-                ev = torch.cuda.Event()
-                ev.record(aux)
-                events.append(ev)
-        out = self.decoder(global_feature, _StreamedFmaps(fmaps, events))
-        main.wait_stream(aux)
-        for f in fmaps:
-            f[0].record_stream(main)
+                fmaps.publish(self.mid_model.level(i, img_fmaps, N))
+            return list(fmaps)
+        side = fork(img.device, 'aux', mid_levels)
+        out = self.decoder(global_feature, fmaps)
+        join(side)
         return out
 
 

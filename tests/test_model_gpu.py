@@ -323,3 +323,37 @@ def test_mano_layer_backward_matches_reference_golden_and_oracle():
     v, j = layer(*z)
     (v.sum() + j.sum()).backward()
     assert z[1].grad.shape == (0, 45)
+
+
+@pytest.mark.parametrize('variant', ['resnet50', 'graph'])
+def test_train_step_launches_only_on_registered_side_streams(variant):
+    """Every kernel of a train-mode forward + backward is launched on the caller's stream or on a side stream registered in
+    ops.STEP_STREAMS: train.TrainStep's overlapped gradient all-reduce waits on exactly those streams.  The forward forks onto the
+    five side streams (left / right hand, two image-grid encoders, the convolution-side aux stream), none of them serialised."""
+    from renderih_b200 import _lib, ops
+    from renderih_b200.model import load_model
+    from renderih_b200.myhand import load_graph_model
+    a = rih_assets.synthetic_assets(0)
+    if variant == 'graph':
+        model = load_graph_model(None, assets=a, mano_assets={s: rih_assets.synthetic_mano(0, s) for s in ('left', 'right')})
+    else:
+        model = load_model(assets=a)
+    model.load_state_dict(fixtures.init_state_dict(model.state_dict()))
+    model = model.cuda().train()
+    img = fixtures.make_image(2).cuda()
+    caller = torch.cuda.current_stream().cuda_stream or 0
+    _lib.TRACE = []
+    try:
+        result, _, _, other = model(img)
+        fwd = {args[-1] or 0 for _, args, _, _ in _lib.TRACE}
+        loss = sum(result['verts3d'][s].sum() + result['verts2d'][s].sum() for s in ('left', 'right'))
+        loss = loss + sum(other[k].sum() for k in ('hms', 'mask', 'dense') if k in other)
+        loss.backward()
+        launched = {args[-1] or 0 for _, args, _, _ in _lib.TRACE}
+    finally:
+        _lib.TRACE = None
+    registered = set(ops.STEP_STREAMS)
+    assert launched <= registered | {caller}, (variant, launched - registered - {caller})
+    wgrad = {st.cuda_stream for st in ops._WG['streams'].values()}
+    side = fwd - {caller} - wgrad
+    assert len(side) == 5 and side <= registered, (variant, side)
