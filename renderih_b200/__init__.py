@@ -30,6 +30,10 @@ Public API mirrors the reference modules it replaces:
                                             (collision.py: per-frame count of intersecting face pairs between the two hand meshes)
     ValidJudger, get_valid_rate         <-  pose_data_optimize/Ver2Code/ValidJudge/ValidJudger.py, GetValidRate.py (valid_judge.py:
                                             the joint-limit validity rate of both hands)
+    HandPoseConverter, HandPoseArguer, PoseArguer, convert_annotations, argue_data, reconvert_optimized, birth_data
+                                        <-  pose_data_optimize/scripts/HandPoseConverter.py, HandPoseArguer.py, Ver2Code/NatureJudge/
+                                            PoseArgue.py, data_birth.py, data/template_{0,1,3}_*.py (pose_data.py: euler / MANO
+                                            quaternion / axis-angle conversions and pose augmentation, one launch per batch)
 """
 from . import _build
 
@@ -79,6 +83,9 @@ def __getattr__(name):
     if name in ('ValidJudger', 'get_valid_rate'):
         from . import valid_judge
         return getattr(valid_judge, name)
+    if name in ('HandPoseConverter', 'HandPoseArguer', 'PoseArguer', 'convert_annotations', 'argue_data', 'reconvert_optimized', 'birth_data'):
+        from . import pose_data
+        return getattr(pose_data, name)
     if name in ('load_cfg', 'get_cfg_defaults'):
         from . import config
         return getattr(config, name)
