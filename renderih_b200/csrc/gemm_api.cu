@@ -82,8 +82,8 @@ RIH_API int rih_set_wgrad_wide(int on) { tc::set_wgrad_wide(on); return 0; }
 //          from shared memory into registers and multiply it with the register-A form of wgmma; only the input operand is transposed in shared memory.
 //   bit 1: the input gradients with at least 128 input channels / in-features (rih_conv2d_dgrad, rih_linear_dgrad) are computed transposed,
 //          dX^T = W^T dY^T: the weights are read into registers and dY is a K-major operand, so nothing is transposed in shared memory and the
-//          TF32 convolution kernels drop the preparation warpgroup.  Every other MN-major A operand (1x1 convolution and Linear weight gradients,
-//          attention dK / dV) is read into registers too.
+//          TF32 convolution kernels drop the preparation warpgroup.  Every other MN-major A operand (1x1 convolution and Linear weight gradients)
+//          is read into registers too.
 // Cleared bits select the shared-memory transpose by the preparation warpgroup (rih_set_gemm_rs(1) = the kernel choices before bit 1 existed).
 // Same products in the same k order: results agree bitwise or to fp32 reordering of the accumulation.
 RIH_API int rih_set_gemm_rs(int bits) { tc::set_gemm_rs(bits); return 0; }

@@ -166,8 +166,6 @@ struct Epilogue {
   unsigned long long site; uint32_t thresh; float inv_keep;
   float scale;                                 // accumulator scale applied first (1 = none; bias-compensated truncating TF32 uses 1 + 7.05e-4)
   double* stats;                               // optional [2*N] column sum / sum of squares of the stored values (fused BatchNorm statistics)
-  int batch_heads;                             // > 0: batched (attention) GEMM on the tensor-core path -- tile batch z addresses the operands / output as
-                                               // 4-D tensors; token matrices use (head, batch) = (z % batch_heads, z / batch_heads), score matrices (z, 0); bit 30 set = output is a score matrix
   int s2_w2, s2_h2, s2_ph, s2_pw;              // tensor-core stride-2 dgrad (s2_w2 > 0): the tile's 128 rows are pixels (n, i, j) of the half-resolution grid
                                                // s2_h2 x s2_w2; they are stored to input pixels (2 i + s2_ph, 2 j + s2_pw) through an element-strided 4-D map
   int kb_rotate;                               // tensor-core persistent kernel: start each tile's k loop at a tile-dependent k-block and wrap around (rih_set_k_rotation)
@@ -203,7 +201,7 @@ struct Epilogue {
 };
 static inline Epilogue make_epilogue(float* c, int ldc, int M, int N, const float* bias, int relu, int mode) {
   Epilogue e; e.c = c; e.ldc = ldc; e.M = M; e.N = N; e.bias = bias; e.relu = relu; e.mode = mode;
-  e.res = nullptr; e.ldres = 0; e.seed_ptr = nullptr; e.site = 0; e.thresh = 0; e.inv_keep = 1.f; e.stats = nullptr; e.scale = 1.f; e.nv_pad = 0; e.nv_real = 0; e.batch_heads = 0; e.s2_w2 = 0; e.s2_h2 = 0; e.s2_ph = 0; e.s2_pw = 0; e.kb_rotate = 0; e.reverse = 0; e.a_policy = 0ull;
+  e.res = nullptr; e.ldres = 0; e.seed_ptr = nullptr; e.site = 0; e.thresh = 0; e.inv_keep = 1.f; e.stats = nullptr; e.scale = 1.f; e.nv_pad = 0; e.nv_real = 0; e.s2_w2 = 0; e.s2_h2 = 0; e.s2_ph = 0; e.s2_pw = 0; e.kb_rotate = 0; e.reverse = 0; e.a_policy = 0ull;
   e.col_scale = nullptr; e.col_shift = nullptr; e.affine_post = 0; e.relu_post = 0; e.opt = 7;
   return e;
 }

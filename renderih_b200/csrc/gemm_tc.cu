@@ -1,6 +1,5 @@
 // Host launchers + C-ABI for the wgmma TF32 GEMM / implicit-GEMM convolution (see gemm_tc.cuh).
 #include "gemm_tc.cuh"
-#include "bgemm.cuh"
 
 namespace rih {
 namespace tc {
@@ -153,7 +152,7 @@ void set_tma_grouped(int on) { g_tma_grouped = on & 7; }       // bit 0: rank-3 
 static int g_epi_opt = 7;        // Epilogue::opt of every launch (rih_set_epilogue_opt)
 void set_epilogue_opt(int v) { g_epi_opt = v & 7; }
 static int g_gemm_rs = 3;        // register-A main loops (rih_set_gemm_rs): bit 0 = the 3x3 / strided convolution weight gradients and the stem's,
-                                 // bit 1 = transposed-output input gradients (dgrad_t) and every other MN-major A operand (dense and batched)
+                                 // bit 1 = transposed-output input gradients (dgrad_t) and every other MN-major A operand
 void set_gemm_rs(int bits) { g_gemm_rs = bits & 3; }
 static int g_tma_res = 1;        // residual rows read by the TMA-store epilogue (0: GEMMs with a residual use per-thread global stores, as before)
 void set_tma_res(int on) { g_tma_res = on ? 1 : 0; }
@@ -163,7 +162,7 @@ static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep,
   // TMA-store epilogue whenever the output is a 16-byte aligned matrix (a residual is read back row-wise by the epilogue threads when it is aligned too)
   CUtensorMap tc_;
   int tma_epi = 0;
-  if (c_map) {       // caller-built output map (3-D wgrad view, batched heads); only the persistent TMA-store epilogue understands it
+  if (c_map) {       // caller-built output map (3-D wgrad view); only the persistent TMA-store epilogue understands it
     if (!g_persistent) { set_error("gemm_tc: output-map override needs the persistent kernel"); return 1; }
     tc_ = *c_map;
     tma_epi = 1;
@@ -176,7 +175,7 @@ static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep,
   }
   if (ep.col_scale && ep.bias) { set_error("gemm_tc: a folded per-column affine and a bias cannot be combined (fold the bias into the shift)"); return 1; }
   if (OUT_T && (!c_map || ep.bias || ep.relu || ep.res || ep.stats || ep.thresh || ep.col_scale || ep.relu_post || ep.mode > 1 || ep.nv_pad ||
-                ep.batch_heads || splits != 1)) {
+                splits != 1)) {
     set_error("gemm_tc: the transposed-output epilogue only scales and stores / accumulates (no bias, activation, residual, dropout, statistics, split-K)");
     return 1;
   }
@@ -300,70 +299,6 @@ int gemm_tf32(const float* a, long long lda, int a_mn, const float* b, long long
 #undef RIH_TC_CASE
   set_error("gemm_tf32: unsupported configuration");
   return 1;
-}
-
-// ---------------------------------------------------------------- batched per-head GEMMs of the attention core
-static int make_tmap_batched(CUtensorMap* map, const BOperand& o, int B, int H, int box_rows, bool atom32) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return 1; }
-  if ((reinterpret_cast<uintptr_t>(o.p) & 15) || (o.ld % 4) || (o.tok && o.cols % 4)) { set_error("attention operand: base / stride / head dim not 16-byte aligned"); return 1; }
-  cuuint64_t dims[4], strides[3];
-  cuuint32_t box[4], estr[4] = {1u, 1u, 1u, 1u};
-  if (o.tok) {   // element (b, h, s, k) at p + (b * S + s) * ld + h * d + k
-    dims[0] = (cuuint64_t)o.cols; dims[1] = (cuuint64_t)H; dims[2] = (cuuint64_t)o.rows; dims[3] = (cuuint64_t)B;
-    strides[0] = (cuuint64_t)o.cols * 4; strides[1] = (cuuint64_t)o.ld * 4; strides[2] = (cuuint64_t)o.rows * o.ld * 4;
-    box[0] = 32u; box[1] = 1u; box[2] = (cuuint32_t)box_rows; box[3] = 1u;
-  } else {       // element (z, r, c) at p + (z * rows + r) * ld + c
-    dims[0] = (cuuint64_t)o.cols; dims[1] = (cuuint64_t)o.rows; dims[2] = (cuuint64_t)B * H; dims[3] = 1;
-    strides[0] = (cuuint64_t)o.ld * 4; strides[1] = (cuuint64_t)o.rows * o.ld * 4; strides[2] = (cuuint64_t)B * H * o.rows * o.ld * 4;
-    box[0] = 32u; box[1] = (cuuint32_t)box_rows; box[2] = 1u; box[3] = 1u;
-  }
-  CUresult r = CUDA_SUCCESS;
-  for (int attempt = 0; attempt < 2; ++attempt) {
-    r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(o.p), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_ERROR_INVALID_CONTEXT) break;
-    cudaFree(0);
-  }
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(batched, tok=%d) failed (%d) rows=%d cols=%d ld=%lld B=%d H=%d", o.tok, (int)r, o.rows, o.cols, o.ld, B, H); return 1; }
-  return 0;
-}
-
-// C[z] = scale * op(A[z]) op(B[z])^T for every head z = b * H + h, as ONE persistent launch: the tile loop runs over (n, m, z).
-//   a_mn / b_mn = 0: operand stored [rows = M|N, cols = K] (K-major); 1: stored [rows = K, cols = M|N] (MN-major).
-int bgemm_tf32(const BOperand& a, int a_mn, const BOperand& b, int b_mn, const BOperand& c, int B, int H, int M, int N, int K, float scale, cudaStream_t s) {
-  if (M <= 0 || N <= 0 || K <= 0 || B * H <= 0) return 0;
-  if (!g_persistent) { set_error("bgemm_tf32 needs the persistent kernel"); return 1; }
-  const int BN = (N > 64) ? 128 : 64;
-  CUtensorMap ta, tb, tcm;
-  if (make_tmap_batched(&ta, a, B, H, a_mn ? 32 : BM, a_mn != 0)) return 1;
-  if (make_tmap_batched(&tb, b, B, H, b_mn ? 32 : BN, b_mn != 0)) return 1;
-  if (make_tmap_batched(&tcm, c, B, H, BM, false)) return 1;
-  Epilogue ep = make_epilogue(const_cast<float*>(c.p), (int)c.ld, M, N, nullptr, 0, 0);
-  ep.batch_heads = H | (c.tok ? 0 : (1 << 30));
-  const int num_kb = cdiv(K, BK);
-  const float keep = g_scale;
-  g_scale = scale * g_scale;     // launch_cfg copies g_scale into ep.scale
-  int rc = 1;
-  bool matched = false;
-#define RIH_BG_CASE(bn, am, bm)                                                                            \
-  if (!matched && BN == bn && a_mn == am && b_mn == bm) {                                                  \
-    BatchedProducer<bn, am != 0, bm != 0> prod{H, a.tok, b.tok}; matched = true;                            \
-    rc = launch_cfg<bn, am != 0, bm != 0>(ta, tb, ep, prod, M, N, num_kb, B * H, num_kb, s, &tcm);           \
-  }
-  // MN-major A (attention dK, dV): read into registers by the consumers (rih_set_gemm_rs bit 1)
-#define RIH_BG_CASE_RS(bn)                                                                                          \
-  if (!matched && (g_gemm_rs & 2) && BN == bn && a_mn == 1 && b_mn == 1) {                                          \
-    BatchedProducer<bn, true, true> prod{H, a.tok, b.tok}; matched = true;                                          \
-    rc = launch_cfg<bn, true, true, BatchedProducer<bn, true, true>, true>(ta, tb, ep, prod, M, N, num_kb, B * H, num_kb, s, &tcm); \
-  }
-  RIH_BG_CASE_RS(128) RIH_BG_CASE_RS(64)
-#undef RIH_BG_CASE_RS
-  RIH_BG_CASE(128, 0, 0) RIH_BG_CASE(64, 0, 0) RIH_BG_CASE(128, 0, 1) RIH_BG_CASE(64, 0, 1) RIH_BG_CASE(128, 1, 1) RIH_BG_CASE(64, 1, 1)
-#undef RIH_BG_CASE
-  g_scale = keep;
-  if (!matched) set_error("bgemm_tf32: unsupported operand majors (a_mn=%d b_mn=%d)", a_mn, b_mn);
-  return rc;
 }
 
 static int g_s2_direct = 1;      // stride-2 convolutions through element-strided tensor maps (no parity-stacked / zero-inserted copies); rih_set_s2_direct

@@ -225,40 +225,6 @@ struct DenseProducer {
   }
 };
 
-// Batched (per attention head) GEMM operands as 4-D tensors, tile batch index z = b * H + h:
-//   token matrix  T[B*S, ld], head slice of width d : dims {d, H, S, B}    -> coordinates (col, z % H, row, z / H)
-//   score matrix  P[B*H, R, C] (row stride padded)   : dims {C, R, B*H, 1}  -> coordinates (col, row, z, 0)
-// Rows / columns of a 128 x BN tile that stick out of ONE head's matrix are zero-filled by the TMA unit (they never alias the next
-// head, because head and batch are separate tensor dimensions), so Sq = 63 ... 316 and d = 16 need no padding copies.
-template <int BN, bool A_MN, bool B_MN>
-struct BatchedProducer {
-  static constexpr bool WIDE_OK = A_MN || B_MN;
-  __device__ __forceinline__ void set_policy(unsigned long long) {}
-  int H;          // heads per batch image
-  int a_tok, b_tok;   // operand is a token matrix (1) or a score matrix (0)
-  // token matrix map dims {d, H, S, B} (strides ascending), score matrix map dims {C, R, B*H, 1}
-  __device__ __forceinline__ void ld4(void* dst, const CUtensorMap* m, int tok, int col, int row, int z, uint64_t* bar) const {
-    if (tok) tma_load_4d(dst, m, col, z % H, row, z / H, bar);
-    else tma_load_4d(dst, m, col, row, z, 0, bar);
-  }
-  template <bool W>
-  __device__ __forceinline__ void load(const CUtensorMap* ta, const CUtensorMap* tb, int kb, int m0, int n0, int z, uint8_t* sa, uint8_t* sb, uint64_t* bar, int lane) const {
-    const int k0 = kb * BK;
-    if constexpr (!A_MN) { if (!W || lane == 0) ld4(sa, ta, a_tok, k0, m0, z, bar); }
-    else if constexpr (W) { if (lane < BM / 32) ld4(sa + lane * (BK * 128), ta, a_tok, m0 + lane * 32, k0, z, bar); }
-    else {
-#pragma unroll
-      for (int c = 0; c < BM / 32; ++c) ld4(sa + c * (BK * 128), ta, a_tok, m0 + c * 32, k0, z, bar);
-    }
-    if constexpr (!B_MN) { if (!W || lane == BM / 32) ld4(sb, tb, b_tok, k0, n0, z, bar); }
-    else if constexpr (W) { const int c = lane - BM / 32; if (c >= 0 && c < BN / 32) ld4(sb + c * (BK * 128), tb, b_tok, n0 + c * 32, k0, z, bar); }
-    else {
-#pragma unroll
-      for (int c = 0; c < BN / 32; ++c) ld4(sb + c * (BK * 128), tb, b_tok, n0 + c * 32, k0, z, bar);
-    }
-  }
-};
-
 struct ConvTcGeom {
   int Cin, Cout, R, S, pad;
   int H, W, Ho, Wo;        // input / output spatial size (stride 1 only)
@@ -695,8 +661,7 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
   __syncthreads();
   pdl_wait();                  // prologue done (barriers, descriptors): from here on the kernel reads what its stream predecessor wrote
 
-  // third tile coordinate z: split-K slice (kb_beg = z * kb_per_split), or -- batched GEMM (ep.batch_heads != 0) -- the batch index
-  const bool batched = ep.batch_heads != 0;
+  // third tile coordinate z: split-K slice (kb_beg = z * kb_per_split)
   auto tile_coords = [&](int t, int& m0, int& n0, int& kb_beg, int& nkb, int& z) {
     if (ep.reverse) t = total_tiles - 1 - t;          // serpentine traversal across consecutive kernels (rih_set_traversal)
     int mi, ni;
@@ -712,8 +677,8 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
       z = r / tiles_m;
     }
     m0 = mi * BM; n0 = ni * BN;
-    kb_beg = batched ? 0 : z * kb_per_split;
-    nkb = batched ? num_kb_total : min(num_kb_total - kb_beg, kb_per_split);
+    kb_beg = z * kb_per_split;
+    nkb = min(num_kb_total - kb_beg, kb_per_split);
   };
 
   if (warp == 0) {
@@ -795,8 +760,8 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
       }
     };
     const bool do_stats = !OUT_T && ep.stats != nullptr;
-    const bool use_res = !OUT_T && tma_epi && ep.res != nullptr && !batched && !ep.nv_pad && (ep.opt & 1);
-    const bool use_cv = !OUT_T && tma_epi && !batched && !ep.nv_pad && (ep.bias != nullptr || ep.col_scale != nullptr) && (ep.opt & 2);
+    const bool use_res = !OUT_T && tma_epi && ep.res != nullptr && !ep.nv_pad && (ep.opt & 1);
+    const bool use_cv = !OUT_T && tma_epi && !ep.nv_pad && (ep.bias != nullptr || ep.col_scale != nullptr) && (ep.opt & 2);
     float4 rcur[8], rnext[8];
     int cv_n0 = -1;
     uint32_t it = 0;
@@ -951,7 +916,6 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
           sc1 = nb / ep.nv_pad; sc0 = nb - sc1 * ep.nv_pad;
           if (sc0 >= ep.nv_real || sc1 * ep.nv_real >= ep.N) continue;      // beyond the tap's channels / beyond the last tap (wide tiles over a padded grid)
         }
-        if (batched && nb >= ep.N) continue;   // e.g. head dim 16 in a 64-wide tile: nothing to store
         if (tma_epi) {
           const float* cmul = use_cv ? colvec + (wg * NCH_WG + (c - wg) / EPI_WG) * 32 : nullptr;
           epilogue_math(v, ep, m, nb, dseed, use_res ? rcur : nullptr, cmul, use_cv ? cmul + BN : nullptr);
@@ -961,11 +925,7 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
           fence_proxy_async();
           epi_bar_sync(wg);
           if (elected) {
-            if (batched) {
-              const int hh = ep.batch_heads & 0x3FFFFFFF;
-              if (ep.batch_heads & (1 << 30)) tma_store_4d(&tmap_c, buf, nb, m0, z, 0);     // score matrix [B*H][M][N]
-              else tma_store_4d(&tmap_c, buf, nb, z % hh, m0, z / hh);                        // head slice of a token matrix
-            } else if (ep.s2_w2) {           // stride-2 dgrad parity class: rows (n, i, j) -> input pixels (2 i + ph, 2 j + pw), element-strided 4-D map
+            if (ep.s2_w2) {           // stride-2 dgrad parity class: rows (n, i, j) -> input pixels (2 i + ph, 2 j + pw), element-strided 4-D map
               const int P2 = ep.s2_h2 * ep.s2_w2;
               const int n_ = row0 / P2, i0 = (row0 - n_ * P2) / ep.s2_w2;
               if (ep.mode == 0) tma_store_4d(&tmap_c, buf, nb, ep.s2_pw, 2 * i0 + ep.s2_ph, n_);

@@ -428,8 +428,8 @@ class AttnFn(Function):
 
 
 class AttnTcFn(Function):
-    """The same attention core with QK^T / PV (and the three backward contractions) on the wgmma tensor cores as batched per-head
-    GEMMs (rih_attn_tc_fwd / rih_attn_tc_bwd); the softmax probabilities [B*H, Sq, Sk] are kept for the backward pass."""
+    """The same attention core on the tensor cores as fused flash-style kernels (rih_attn_tc_fwd / rih_attn_tc_bwd): no score matrix
+    reaches global memory; the forward keeps O and two statistics per query row (row max, 1 / row sum) for the backward pass."""
 
     @staticmethod
     def forward(ctx, q, k, v, B, H, Sq, Sk, p_drop, site, nsplit):
@@ -437,37 +437,33 @@ class AttnTcFn(Function):
         HD = q.shape[1]
         d = HD // H
         assert q.shape[0] == B * Sq and k.shape[0] == B * Sk and v.shape[0] == B * Sk
-        ldp = (Sk + 3) // 4 * 4
         o = torch.empty((B * Sq, HD), device=q.device, dtype=torch.float32)
-        P = torch.empty((B * H, Sq, ldp), device=q.device, dtype=torch.float32)
-        Pd = torch.empty_like(P) if p_drop > 0 else None
+        stats = torch.empty((B * H * Sq, 2), device=q.device, dtype=torch.float32)
         scale = 1.0 / (d ** 0.5)
         sp = seed_state.ptr(q.device) if p_drop > 0 else None
-        call('rih_attn_tc_fwd', _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(o), HD, _p(P), _p(Pd), ldp,
+        call('rih_attn_tc_fwd', _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(o), HD, _p(stats), None, 0,
              B, H, Sq, Sk, d, scale, float(p_drop), sp, site, nsplit, _stream())
-        ctx.save_for_backward(q, k, v, P)
-        ctx.meta = (B, H, Sq, Sk, d, scale, p_drop, site, nsplit, ldp)
+        ctx.save_for_backward(q, k, v, o, stats)
+        ctx.meta = (B, H, Sq, Sk, d, scale, p_drop, site, nsplit)
         return o
 
     @staticmethod
     def backward(ctx, do):
-        q, k, v, P = ctx.saved_tensors
-        B, H, Sq, Sk, d, scale, p_drop, site, nsplit, ldp = ctx.meta
+        q, k, v, o, stats = ctx.saved_tensors
+        B, H, Sq, Sk, d, scale, p_drop, site, nsplit = ctx.meta
         do = _rows(do.contiguous() if do.stride(-1) != 1 else do)
         HD = H * d
         dq = torch.empty((B * Sq, HD), device=do.device, dtype=torch.float32)
         dk = torch.empty((B * Sk, HD), device=do.device, dtype=torch.float32)
         dv = torch.empty((B * Sk, HD), device=do.device, dtype=torch.float32)
-        ws = torch.empty_like(P)
-        Pd = torch.empty_like(P) if p_drop > 0 else None
         sp = seed_state.ptr(do.device) if p_drop > 0 else None
-        call('rih_attn_tc_bwd', _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(do), _ld(do), _p(P), _p(ws), _p(Pd), ldp,
+        call('rih_attn_tc_bwd', _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(do), _ld(do), _p(stats), _p(o), None, HD,
              _p(dq), HD, _p(dk), HD, _p(dv), HD, B, H, Sq, Sk, d, scale, float(p_drop), sp, site, nsplit, _stream())
         return dq, dk, dv, None, None, None, None, None, None, None
 
 
 def attention(q, k, v, B, H, Sq, Sk, p_drop=0.0, impl=None):
-    """impl: None = follow set_gemm_mode (SIMT fused kernel in 'simt' mode, tensor-core batched GEMMs otherwise), 'simt' | 'tc' to force."""
+    """impl: None = follow set_gemm_mode (SIMT fused kernel in 'simt' mode, tensor-core fused kernels otherwise), 'simt' | 'tc' to force."""
     site = seed_state.next_site() if p_drop > 0 else 0
     nsplit = _ATTN['nsplit']
     impl = impl or _ATTN.get('force')
@@ -555,26 +551,24 @@ class AttnProjFn(Function):
         o = torch.empty((Mq, HD), device=dev, dtype=torch.float32)
         scale = 1.0 / (d ** 0.5)
         sp = seed_state.ptr(dev) if p_drop > 0 else None
-        P = Pd = lse = None
-        ldp = (Sk + 3) // 4 * 4
+        stats = lse = None
         if nsplit:
-            P = torch.empty((B * H, Sq, ldp), device=dev, dtype=torch.float32)
-            Pd = torch.empty_like(P) if p_drop > 0 else None
-            call('rih_attn_tc_fwd', _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(o), HD, _p(P), _p(Pd), ldp,
+            stats = torch.empty((B * H * Sq, 2), device=dev, dtype=torch.float32)
+            call('rih_attn_tc_fwd', _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(o), HD, _p(stats), None, 0,
                  B, H, Sq, Sk, d, scale, float(p_drop), sp, site, nsplit, s)
         else:
             lse = torch.empty((B * H * Sq,), device=dev, dtype=torch.float32)
             call('rih_attn_fwd', _p(q), Sq * _ld(q), _ld(q), _p(k), Sk * _ld(k), _ld(k), _p(v), Sk * _ld(v), _ld(v),
                  _p(o), Sq * HD, HD, _p(lse), B, H, Sq, Sk, d, scale, float(p_drop), sp, site, s)
-        ctx.save_for_backward(xq, None if same else xkv, wq, wk, wv, qkv, kvbuf, o, P, lse)
-        ctx.meta = (same, B, H, Sq, Sk, d, scale, p_drop, site, nsplit, ldp)
+        ctx.save_for_backward(xq, None if same else xkv, wq, wk, wv, qkv, kvbuf, o, stats, lse)
+        ctx.meta = (same, B, H, Sq, Sk, d, scale, p_drop, site, nsplit)
         ctx.refs = (bq, bk, bv)
         return o
 
     @staticmethod
     def backward(ctx, do):
-        xq, xkv, wq, wk, wv, qkv, kvbuf, o, P, lse = ctx.saved_tensors
-        same, B, H, Sq, Sk, d, scale, p_drop, site, nsplit, ldp = ctx.meta
+        xq, xkv, wq, wk, wv, qkv, kvbuf, o, stats, lse = ctx.saved_tensors
+        same, B, H, Sq, Sk, d, scale, p_drop, site, nsplit = ctx.meta
         bq, bk, bv = ctx.refs
         if same:
             xkv = xq
@@ -595,9 +589,7 @@ class AttnProjFn(Function):
             dq, dk, dv = dqkv, dkv[:, :HD], dkv[:, HD:]
         sp = seed_state.ptr(dev) if p_drop > 0 else None
         if nsplit:
-            ws = torch.empty_like(P)
-            Pd = torch.empty_like(P) if p_drop > 0 else None
-            call('rih_attn_tc_bwd', _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(do), _ld(do), _p(P), _p(ws), _p(Pd), ldp,
+            call('rih_attn_tc_bwd', _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(do), _ld(do), _p(stats), _p(o), None, HD,
                  _p(dq), _ld(dq), _p(dk), _ld(dk), _p(dv), _ld(dv), B, H, Sq, Sk, d, scale, float(p_drop), sp, site, nsplit, s)
         else:
             call('rih_attn_bwd', _p(q), Sq * _ld(q), _ld(q), _p(k), Sk * _ld(k), _ld(k), _p(v), Sk * _ld(v), _ld(v),

@@ -1,5 +1,7 @@
 """Per-shape timing of the attention core (forward / backward) at the 9 (Sq, Sk, d) shapes of the decoder (SURVEY 8 a2), batch 64 x 4 heads,
-CUDA events, L2 flushed between launches.  usage: python tools/bench_attn.py [--rows-fwd 0|4|8] [--rows-bwd 0|2|4] [--dropout 0.05]"""
+CUDA events, L2 flushed between launches.  Beside each time: the algorithmic HBM traffic of the fused tensor-core core (forward reads
+q, k, v and writes o and 2 floats of row statistics per query row; backward reads q, k, v, o, dO and the statistics and writes dq, dk, dv)
+and the rate that implies.  usage: python tools/bench_attn.py [--rows-fwd 0|4|8] [--rows-bwd 0|2|4] [--dropout 0.05]"""
 import argparse
 import os
 import sys
@@ -50,7 +52,10 @@ def main():
                 tf += e0.elapsed_time(e1) / reps
                 tb += e1.elapsed_time(e2) / reps
         fl = 4.0 * B * H * Sq * Sk * d
-        print('Sq %3d Sk %3d d %2d x%d : fwd %7.1f us (%5.1f TF/s)   bwd %7.1f us (%5.1f TF/s)' % (Sq, Sk, d, calls, tf * 1e3, fl / tf / 1e9, tb * 1e3, 2.5 * fl / tb / 1e9))
+        by_f = 4.0 * B * H * (d * (2 * Sq + 2 * Sk) + 2 * Sq)
+        by_b = 4.0 * B * H * (d * (4 * Sq + 4 * Sk) + 2 * Sq)
+        print('Sq %3d Sk %3d d %2d x%d : fwd %7.1f us (%5.1f TF/s, %5.2f MB, %6.1f GB/s)   bwd %7.1f us (%5.1f TF/s, %5.2f MB, %6.1f GB/s)'
+              % (Sq, Sk, d, calls, tf * 1e3, fl / tf / 1e9, by_f / 1e6, by_f / tf / 1e6, tb * 1e3, 2.5 * fl / tb / 1e9, by_b / 1e6, by_b / tb / 1e6))
         tot_f += tf * calls; tot_b += tb * calls
     print('per training step (24 cores): fwd %.3f ms  bwd %.3f ms' % (tot_f, tot_b))
 
