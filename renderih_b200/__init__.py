@@ -34,6 +34,10 @@ Public API mirrors the reference modules it replaces:
                                         <-  pose_data_optimize/scripts/HandPoseConverter.py, HandPoseArguer.py, Ver2Code/NatureJudge/
                                             PoseArgue.py, data_birth.py, data/template_{0,1,3}_*.py (pose_data.py: euler / MANO
                                             quaternion / axis-angle conversions and pose augmentation, one launch per batch)
+    HeatmapGenerator, cut_img, InterHandLoader, select_data, cut_inter_img, InterHand_dataset, render_data
+                                        <-  dataset/heatmap.py, dataset/dataset_utils.py, utils/dataset_gen/interhand.py,
+                                            rendering_code/step7_gen_annotations.py (dataset_gen.py: batched crops, annotations,
+                                            ori_handdict labels, heatmaps, masks and dense maps)
 """
 from . import _build
 
@@ -86,6 +90,9 @@ def __getattr__(name):
     if name in ('HandPoseConverter', 'HandPoseArguer', 'PoseArguer', 'convert_annotations', 'argue_data', 'reconvert_optimized', 'birth_data'):
         from . import pose_data
         return getattr(pose_data, name)
+    if name in ('HeatmapGenerator', 'cut_img', 'InterHandLoader', 'select_data', 'cut_inter_img', 'InterHand_dataset', 'render_data'):
+        from . import dataset_gen
+        return getattr(dataset_gen, name)
     if name in ('load_cfg', 'get_cfg_defaults'):
         from . import config
         return getattr(config, name)
