@@ -33,39 +33,41 @@ def _drop(x, p, training):
 
 
 # ---------------------------------------------------------------- encoder: models/encoder.py:107-126 + torchvision Bottleneck
-def _bottleneck(x, sd, pre, stride, has_ds, tr):
-    out = F.relu(_bn(F.conv2d(x, sd[pre + '.conv1.weight']), sd, pre + '.bn1', tr))
-    out = F.relu(_bn(F.conv2d(out, sd[pre + '.conv2.weight'], stride=stride, padding=1), sd, pre + '.bn2', tr))
-    out = _bn(F.conv2d(out, sd[pre + '.conv3.weight']), sd, pre + '.bn3', tr)
+# `conv` (default F.conv2d, same signature) replaces every convolution of the encoder functions below, so that a test can run the
+# same graph with convolutions in another arithmetic (e.g. fp64 products of TF32-rounded operands).
+def _bottleneck(x, sd, pre, stride, has_ds, tr, conv=F.conv2d):
+    out = F.relu(_bn(conv(x, sd[pre + '.conv1.weight']), sd, pre + '.bn1', tr))
+    out = F.relu(_bn(conv(out, sd[pre + '.conv2.weight'], stride=stride, padding=1), sd, pre + '.bn2', tr))
+    out = _bn(conv(out, sd[pre + '.conv3.weight']), sd, pre + '.bn3', tr)
     idt = x
     if has_ds:
-        idt = _bn(F.conv2d(x, sd[pre + '.downsample.0.weight'], stride=stride), sd, pre + '.downsample.1', tr)
+        idt = _bn(conv(x, sd[pre + '.downsample.0.weight'], stride=stride), sd, pre + '.downsample.1', tr)
     return F.relu(out + idt)
 
 
-def _simple_decoder(x, sd, pre, tr):
+def _simple_decoder(x, sd, pre, tr, conv=F.conv2d):
     """ResNetSimple_decoder.forward, models/encoder.py:58-64: flat 1x1 then 3x (bilinear x2, 3x3 conv, ReLU, BN)."""
     fmaps = []
-    x = _bn(F.relu(F.conv2d(x, sd[pre + '.models.0.0.weight'])), sd, pre + '.models.0.2', tr)
+    x = _bn(F.relu(conv(x, sd[pre + '.models.0.0.weight'])), sd, pre + '.models.0.2', tr)
     fmaps.append(x)
     for i in (1, 2, 3):
         x = F.interpolate(x, scale_factor=2, mode='bilinear', align_corners=True)
-        x = _bn(F.relu(F.conv2d(x, sd['%s.models.%d.1.weight' % (pre, i)], padding=1)), sd, '%s.models.%d.3' % (pre, i), tr)
+        x = _bn(F.relu(conv(x, sd['%s.models.%d.1.weight' % (pre, i)], padding=1)), sd, '%s.models.%d.3' % (pre, i), tr)
         fmaps.append(x)
-    out = F.conv2d(x, sd[pre + '.final_layer.weight'], sd[pre + '.final_layer.bias'])
+    out = conv(x, sd[pre + '.final_layer.weight'], sd[pre + '.final_layer.bias'])
     return out, fmaps
 
 
-def resnet_trunk(sd, img, tr, blocks=(3, 4, 6, 3)):
+def resnet_trunk(sd, img, tr, blocks=(3, 4, 6, 3), conv=F.conv2d):
     """torchvision ResNet-50 trunk as driven by ResNetSimple.forward (models/encoder.py:107-118 == common/myhand/encoder_lijun.py:91-104)"""
     p = 'encoder.resnet'
-    x = F.relu(_bn(F.conv2d(img, sd[p + '.conv1.weight'], stride=2, padding=3), sd, p + '.bn1', tr))
+    x = F.relu(_bn(conv(img, sd[p + '.conv1.weight'], stride=2, padding=3), sd, p + '.bn1', tr))
     x = F.max_pool2d(x, 3, 2, 1)
     feats = []
     for li, nb in enumerate(blocks):
         for bi in range(nb):
             stride = 2 if (bi == 0 and li > 0) else 1
-            x = _bottleneck(x, sd, '%s.layer%d.%d' % (p, li + 1, bi), stride, bi == 0, tr)
+            x = _bottleneck(x, sd, '%s.layer%d.%d' % (p, li + 1, bi), stride, bi == 0, tr, conv=conv)
         feats.append(x)
     return feats[::-1]          # [x1 (8x8), x2, x3, x4 (64x64)]
 
@@ -76,23 +78,23 @@ def graph_mid_forward(sd, img_f, tr):
     return gf, [_bn(F.relu(F.conv2d(img_f[i], sd['mid_model.convs.%d.0.weight' % i])), sd, 'mid_model.convs.%d.2' % i, tr) for i in range(4)]
 
 
-def encoder_forward(sd, img, tr, blocks=(3, 4, 6, 3)):
+def encoder_forward(sd, img, tr, blocks=(3, 4, 6, 3), conv=F.conv2d):
     p = 'encoder.resnet'
-    x = F.relu(_bn(F.conv2d(img, sd[p + '.conv1.weight'], stride=2, padding=3), sd, p + '.bn1', tr))
+    x = F.relu(_bn(conv(img, sd[p + '.conv1.weight'], stride=2, padding=3), sd, p + '.bn1', tr))
     x = F.max_pool2d(x, 3, 2, 1)
     feats = []
     for li, nb in enumerate(blocks):
         for bi in range(nb):
             stride = 2 if (bi == 0 and li > 0) else 1
-            x = _bottleneck(x, sd, '%s.layer%d.%d' % (p, li + 1, bi), stride, bi == 0, tr)
+            x = _bottleneck(x, sd, '%s.layer%d.%d' % (p, li + 1, bi), stride, bi == 0, tr, conv=conv)
         feats.append(x)
     x4, x3, x2, x1 = feats
-    hms, hms_f = _simple_decoder(x1, sd, 'encoder.hms_decoder', tr)
-    out, dp_f = _simple_decoder(x1, sd, 'encoder.dp_decoder', tr)
+    hms, hms_f = _simple_decoder(x1, sd, 'encoder.hms_decoder', tr, conv=conv)
+    out, dp_f = _simple_decoder(x1, sd, 'encoder.dp_decoder', tr, conv=conv)
     return hms, out[:, :2], out[:, 2:], [x1, x2, x3, x4], hms_f, dp_f
 
 
-def mid_forward(sd, img_f, hms_f, dp_f, tr):
+def mid_forward(sd, img_f, hms_f, dp_f, tr, conv=F.conv2d):
     """resnet_mid.forward, models/encoder.py:165-173 (conv1x1 helper = Conv -> ReLU -> BN, model_zoo/__init__.py:56-62)"""
     gf = F.adaptive_avg_pool2d(img_f[0], 1).flatten(1)
     fmaps = []
@@ -100,7 +102,7 @@ def mid_forward(sd, img_f, hms_f, dp_f, tr):
         x = torch.cat((hms_f[i], dp_f[i]), 1)
         if i > 0:
             x = torch.cat((x, img_f[i]), 1)
-        fmaps.append(_bn(F.relu(F.conv2d(x, sd['mid_model.convs.%d.0.weight' % i])), sd, 'mid_model.convs.%d.2' % i, tr))
+        fmaps.append(_bn(F.relu(conv(x, sd['mid_model.convs.%d.0.weight' % i])), sd, 'mid_model.convs.%d.2' % i, tr))
     return gf, fmaps
 
 
@@ -113,10 +115,10 @@ def _count(sd, pre):
     return n
 
 
-def _basic_block(x, sd, pre, tr):
+def _basic_block(x, sd, pre, tr, conv=F.conv2d):
     """BasicBlock.forward, model_zoo/hrnet.py:41-58 (branch blocks never carry a downsample: in == out channels)"""
-    out = F.relu(_bn(F.conv2d(x, sd[pre + '.conv1.weight'], padding=1), sd, pre + '.bn1', tr))
-    out = _bn(F.conv2d(out, sd[pre + '.conv2.weight'], padding=1), sd, pre + '.bn2', tr)
+    out = F.relu(_bn(conv(x, sd[pre + '.conv1.weight'], padding=1), sd, pre + '.bn1', tr))
+    out = _bn(conv(out, sd[pre + '.conv2.weight'], padding=1), sd, pre + '.bn2', tr)
     return F.relu(out + x)
 
 

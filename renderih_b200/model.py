@@ -193,11 +193,28 @@ class ResNetSimple(nn.Module):
 
     def trunk(self, img, fold_done=False):
         """stem + layer1..4 (encoder.py:107-118) -> [x1 (8x8), x2, x3, x4 (64x64)] as (NHWC rows, H) pairs."""
-        N, C, H, W = img.shape
-        assert H == W
+        N = img.shape[0]
         r = self.resnet
         if not self.training and not fold_done:
             ops.bn_fold_refresh(self)        # inference: one launch folds every BatchNorm of the encoder for the conv epilogues
+        x, H = self.stem(img)
+        feats = []
+        for layer in (r.layer1, r.layer2, r.layer3, r.layer4):
+            for blk in layer:
+                x, H = self._bottleneck(blk, x, N, H) if self.expansion == 4 else self._basic(blk, x, N, H)
+            # this layer's output gradient is complete exactly when every later layer / head has been back-propagated (train.TrainStep
+            # starts the gradient all-reduce of those parameters then)
+            ops.backward_marker(x, 'encoder.resnet.layer%d' % (len(feats) + 1))
+            feats.append((x, H))
+        x4, x3, x2, x1 = feats
+        return [x1, x2, x3, x4]
+
+    def stem(self, img):
+        """conv1 + bn1 + ReLU + max-pool (encoder.py:107-110) in one of three forms: the implicit-GEMM stem_conv (tensor-core modes, 256 x 256
+        images, no image gradient), _stem's im2col GEMM (no image gradient) or _conv_bn (the image needs a gradient).  -> (NHWC rows, H)"""
+        N, C, H, W = img.shape
+        assert H == W
+        r = self.resnet
         if not img.requires_grad and ops.stem_supported(H, W):
             # conv1 straight from the NCHW image: zero-bordered NHWC4 copy + wgmma implicit GEMM (no im2col buffer), train and eval mode
             conv, bn = r.conv1, r.bn1
@@ -212,17 +229,7 @@ class ResNetSimple(nn.Module):
             x = ops.nchw_to_nhwc(img)
             x, H = self._stem(x, N, H, img.requires_grad)
         x = ops.maxpool3x3s2(x, N, H, H)
-        H = (H - 1) // 2 + 1
-        feats = []
-        for layer in (r.layer1, r.layer2, r.layer3, r.layer4):
-            for blk in layer:
-                x, H = self._bottleneck(blk, x, N, H) if self.expansion == 4 else self._basic(blk, x, N, H)
-            # this layer's output gradient is complete exactly when every later layer / head has been back-propagated (train.TrainStep
-            # starts the gradient all-reduce of those parameters then)
-            ops.backward_marker(x, 'encoder.resnet.layer%d' % (len(feats) + 1))
-            feats.append((x, H))
-        x4, x3, x2, x1 = feats
-        return [x1, x2, x3, x4]
+        return x, (H - 1) // 2 + 1
 
     def aux_outputs(self, hms, out, N, Hh):
         """NHWC head outputs -> the NCHW hms / mask / dense maps of encoder.py:121-125."""

@@ -1111,8 +1111,9 @@ class BatchNormFn(Function):
         # ONE launch: mean / rstd from the column sums (or the running statistics in eval mode), running-stat + num_batches_tracked
         # update, normalise (+res)(+relu)
         # the ReLU mask of a residual block cannot be recomputed from x alone: the forward kernel records it as one byte per channel quad
-        # (1/16 of the output's bytes), which the two backward passes read instead of the output; otherwise it is recomputed from x
-        mask = torch.empty((M, C // 4), device=dev, dtype=torch.uint8) if (relu and res is not None and ctx.needs_input_grad[0]) else None
+        # (1/16 of the output's bytes), which the two backward passes read instead of the output; otherwise it is recomputed from x.
+        # Every gradient of a residual block passes that gate (dres, dgamma and dbeta too), so it is recorded whenever a backward may run.
+        mask = torch.empty((M, C // 4), device=dev, dtype=torch.uint8) if (relu and res is not None and any(ctx.needs_input_grad)) else None
         call('rih_bn_forward', _p(x), _ld(x), _p(stats) if training else None, M, C, float(eps), float(momentum), _p(gamma), _p(beta),
              _p(res), _ld(res) if res is not None else 0, _p(y), C, int(relu), _p(mask), _p(mean), _p(rstd), _p(rmean), _p(rvar),
              _p(tracked) if training else None, s)
