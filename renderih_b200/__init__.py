@@ -38,6 +38,9 @@ Public API mirrors the reference modules it replaces:
                                         <-  dataset/heatmap.py, dataset/dataset_utils.py, utils/dataset_gen/interhand.py,
                                             rendering_code/step7_gen_annotations.py (dataset_gen.py: batched crops, annotations,
                                             ori_handdict labels, heatmaps, masks and dense maps)
+    JointFitter, adaptive_IK, mat2aa, get_3djoints, get_3djoints_batch, read_worldpos_csv, convert
+                                        <-  utils/mano_from_3djoint/convert2mano.py, AIK.py, utils.py (mano_from_3djoint.py: fitting MANO
+                                            to motion-capture joints, every frame and both hands in one batched run)
 """
 from . import _build
 
@@ -93,6 +96,9 @@ def __getattr__(name):
     if name in ('HeatmapGenerator', 'cut_img', 'InterHandLoader', 'select_data', 'cut_inter_img', 'InterHand_dataset', 'render_data'):
         from . import dataset_gen
         return getattr(dataset_gen, name)
+    if name in ('JointFitter', 'adaptive_IK', 'mat2aa', 'get_3djoints', 'get_3djoints_batch', 'read_worldpos_csv', 'convert'):
+        from . import mano_from_3djoint
+        return getattr(mano_from_3djoint, name)
     if name in ('load_cfg', 'get_cfg_defaults'):
         from . import config
         return getattr(config, name)
