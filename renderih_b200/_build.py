@@ -41,42 +41,6 @@ def needs_build():
         return f.read().strip() != _digest()
 
 
-def variant_path(name):
-    return os.path.join(HERE, 'librih_b200_%s.so' % name)
-
-
-def build_variant(name, defines, verbose=False):
-    """Build an A/B variant of the library with extra -D defines (compile-time tuning knobs of csrc/gemm_tc.cuh); only the translation units
-    that include gemm_tc.cuh are recompiled, the rest of the objects are shared with the main build.  Selected at run time with
-    RIH_LIB_VARIANT=<name>.  -> path"""
-    build()
-    nvcc = shutil.which('nvcc') or '/usr/local/cuda/bin/nvcc'
-    objdir = os.path.join(HERE, 'csrc', 'build')
-    vdir = os.path.join(objdir, 'variant_' + name)
-    os.makedirs(vdir, exist_ok=True)
-    common = [nvcc] + ARCH_FLAGS + ['-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC,-fvisibility=hidden',
-                                    '-I', CSRC, '-I', os.path.join(HERE, '..', 'include')] + ['-D%s' % d for d in defines]
-    objs, procs = [], []
-    for src in _sources():
-        with open(os.path.join(CSRC, src)) as f:
-            uses = 'gemm_tc.cuh' in f.read()
-        if uses:
-            obj = os.path.join(vdir, src[:-3] + '.o')
-            procs.append((src, subprocess.Popen(common + ['-c', os.path.join(CSRC, src), '-o', obj], stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))
-        else:
-            obj = os.path.join(objdir, src[:-3] + '.o')
-        objs.append(obj)
-    for src, p in procs:
-        out, _ = p.communicate()
-        if p.returncode != 0:
-            raise RuntimeError('nvcc failed on %s (variant %s):\n%s' % (src, name, out.decode()))
-    path = variant_path(name)
-    r = subprocess.run([nvcc] + ARCH_FLAGS + ['-shared', '-o', path] + objs + ['-lcuda'], stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
-    if r.returncode != 0:
-        raise RuntimeError('link failed (variant %s):\n%s' % (name, r.stdout.decode()))
-    return path
-
-
 def have_nvcc():
     return os.path.exists(shutil.which('nvcc') or '/usr/local/cuda/bin/nvcc')
 

@@ -43,8 +43,6 @@ def parse_header(path=HEADER):
     return protos
 
 
-SERPENTINE = [os.environ.get('RIH_SERPENTINE', '0') != '0', 0]     # [enabled, current direction]
-SERPENTINE_NAMES = {'rih_conv2d_fwd', 'rih_conv2d_dgrad', 'rih_bn_forward', 'rih_bn_bwd'}
 PDL_DEFAULT = '0'     # flipped to '1' once validated on hardware (A/B in bench.py)
 STREAM_LAST = set()   # entry points whose last parameter is the CUDA stream to launch on (every kernel-launching one)
 TRACE = None          # measurement hook (bench.py): when set to a list, every launching call is bracketed by CUDA events recorded on ITS stream
@@ -62,12 +60,7 @@ def load():
     if _lib is not None:
         return _lib
     path = _build.LIB_PATH
-    variant = os.environ.get('RIH_LIB_VARIANT')
-    if variant:             # an A/B build with other compile-time knobs (renderih_b200/_build.build_variant); must exist already
-        path = _build.variant_path(variant)
-        if not os.path.exists(path):
-            raise RuntimeError('renderih_b200: library variant %r not built (%s)' % (variant, path))
-    if not variant and _build.needs_build():
+    if _build.needs_build():
         if _build.have_nvcc():
             _build.build()          # compile / link errors propagate: never run a stale library against a newer header
         elif not os.path.exists(path):
@@ -85,15 +78,6 @@ def load():
     _lib = lib
     # programmatic dependent launch for every kernel (csrc/common.cuh); RIH_PDL=0 selects plain stream-ordered launches
     lib.rih_set_pdl(1 if os.environ.get('RIH_PDL', PDL_DEFAULT) != '0' else 0)
-    lib.rih_set_narrow_tiles(1 if os.environ.get('RIH_NARROW_TILES', '0') != '0' else 0)      # measured: 64-wide tiles for small GEMMs cost 1.1 ms of the step
-    lib.rih_set_s2_direct(0 if os.environ.get('RIH_S2_DIRECT', '1') == '0' else 1)
-    lib.rih_set_epilogue_opt(int(os.environ.get('RIH_EPI_OPT', '7')))
-    lib.rih_set_tma_grouped(int(os.environ.get('RIH_TMA_GROUPED', '7')))     # bit 0: train step 30.48 -> 30.07 ms; bit 1 (rank-5 input boxes of the conv wgrad): 30.10 -> 29.83 ms; bit 2 (weight boxes of the conv dgrad): 29.86 -> 29.69 ms
-    lib.rih_set_tma_res(0 if os.environ.get('RIH_TMA_RES', '1') == '0' else 1)
-    lib.rih_set_k_rotation(1 if os.environ.get('RIH_K_ROTATE', '0') != '0' else 0)
-    lib.rih_set_wgrad_wide(int(os.environ.get('RIH_WGRAD_WIDE', '3')))       # bit 1 = wide tiles for padded channel counts too (HRNet-w48 step 70.55 -> 66.97 ms)
-    lib.rih_set_ew_cap(0 if os.environ.get('RIH_EW_CAP', '1') == '0' else 1)
-    lib.rih_set_l2_hints(0 if os.environ.get('RIH_L2_HINTS', '1') == '0' else 1)             # measured: -0.16 ms on the trunk
     return lib
 
 
@@ -101,9 +85,6 @@ def call(name, *args):
     """Invoke a C-ABI entry point; raise RuntimeError(rih_last_error()) on a non-zero status."""
     lib = _lib if _lib is not None else load()
     CALLS[0] += 1
-    if SERPENTINE[0] and name in SERPENTINE_NAMES:      # alternate the traversal direction along the convolution / BatchNorm chain
-        SERPENTINE[1] ^= 1
-        lib.rih_set_traversal(SERPENTINE[1])
     if TRACE is not None and name in STREAM_LAST:
         import torch
         st = torch.cuda.ExternalStream(args[-1]) if args[-1] else torch.cuda.default_stream()

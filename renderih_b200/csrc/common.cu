@@ -4,9 +4,6 @@
 namespace rih {
 static thread_local char g_err[1024] = "";
 int g_pdl = 0;
-int g_reverse = 0;
-int g_l2_hints = 0;
-int g_kb_rotate = 0;
 
 void set_error(const char* fmt, ...) {
   va_list ap;
@@ -30,9 +27,8 @@ int stream_cta_limit(cudaStream_t s, int num_sms) {
   for (int i = 0; i < CAP_SLOTS; ++i) if (g_cap_ctas[i] > 0 && g_cap_stream[i] == s) return g_cap_ctas[i] < num_sms ? g_cap_ctas[i] : num_sms;
   return num_sms;
 }
-int g_ew_cap = 1;
 long long ew_ctas(cudaStream_t s) {
-  if (g_ew_cap) for (int i = 0; i < CAP_SLOTS; ++i) if (g_cap_ctas[i] > 0 && g_cap_stream[i] == s && 3 * g_cap_ctas[i] < 2 * sm_count()) return sm_count() * 4;
+  for (int i = 0; i < CAP_SLOTS; ++i) if (g_cap_ctas[i] > 0 && g_cap_stream[i] == s && 3 * g_cap_ctas[i] < 2 * sm_count()) return sm_count() * 4;
   return sm_count() * 16;
 }
 
@@ -65,23 +61,6 @@ RIH_API int rih_version(void) { return 200; }
 // Programmatic dependent launch for every kernel of the library (see common.cuh): 1 = on, 0 = plain stream-ordered launches.  Scheduling only:
 // results are unchanged (no reference counterpart).
 RIH_API int rih_set_pdl(int on) { rih::g_pdl = on ? 1 : 0; return 0; }
-
-// Traversal direction of the NEXT launches: 1 = the tensor-core GEMM / convolution kernels walk their output tiles, and the BatchNorm passes
-// their rows, from the last to the first.  A consumer that starts where its producer finished finds the most recently written part of an
-// activation (whatever of it fits in the 50 MB L2) still cached; alternating the direction kernel by kernel ("serpentine") keeps that true
-// along a whole chain of layers.  Scheduling only: results are unchanged up to summation order in atomically accumulated statistics.
-RIH_API int rih_set_traversal(int reverse) { rih::g_reverse = reverse ? 1 : 0; return 0; }
-
-// 1 = activations that a GEMM / 1x1 convolution / BatchNorm pass streams through once are loaded with the L2 evict-first priority, so that they do
-// not displace the previous kernel's output (which the next kernel is about to read) from the L2.  Scheduling only.
-// 1 (default) = element-wise kernels launched on a CTA-capped stream (rih_set_stream_cta_limit) use a quarter of their usual grid.  Scheduling only.
-// 1 = every output tile of the tensor-core GEMM / convolution kernels starts its k loop at a tile-dependent k-block and wraps around, so
-// that concurrently running CTAs do not all fetch the same 128-byte slice of their rows at the same time.  Results agree up to fp32
-// summation order inside the tensor core accumulation.
-RIH_API int rih_set_k_rotation(int on) { rih::g_kb_rotate = on ? 1 : 0; return 0; }
-RIH_API int rih_set_ew_cap(int on) { rih::g_ew_cap = on ? 1 : 0; return 0; }
-
-RIH_API int rih_set_l2_hints(int on) { rih::g_l2_hints = on ? 1 : 0; return 0; }
 
 // Device properties probe (used by the host side to fail loudly on a device other than sm_90).
 RIH_API int rih_device_info(int device, int* cc_major, int* cc_minor, int* sm_count, size_t* smem_optin) {

@@ -45,9 +45,6 @@ static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b)
 // 5-15 us kernels).  Nothing before pdl_wait() may touch global memory a predecessor writes.  Under CUDA-graph capture the edges become
 // programmatic dependencies of the graph.  g_pdl == 0: plain launches; griddepcontrol.* are no-ops then.
 extern int g_pdl;
-extern int g_reverse;    // rih_set_traversal: walk tiles / rows from the end (serpentine traversal across consecutive kernels)
-extern int g_kb_rotate;  // rih_set_k_rotation: per-tile rotation of the k-block order in the tensor-core GEMMs
-extern int g_l2_hints;   // rih_set_l2_hints: evict-first loads of streamed activations
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_sync() { pdl_launch_dependents(); pdl_wait(); }

@@ -11,13 +11,9 @@ int gemm_tf32(const float* a, long long lda, int a_mn, const float* b, long long
               int allow_splitk, cudaStream_t s);
 bool conv_tc_supported(const ConvGeom& g, int which);
 void set_nsplit(int n);
-void set_narrow_small(int on);
-void set_wgrad_wide(int on);
 void set_s2_direct(int on);
-void set_tma_res(int on);
 void set_gemm_rs(int bits);
 void set_epilogue_opt(int v);
-void set_tma_grouped(int on);
 int s2_direct();
 void set_acc_scale(float s);
 extern int g_stats_fused;
@@ -52,14 +48,6 @@ RIH_API int rih_set_stream_cta_limit(cudaStream_t stream, int ctas) {
   RIH_REQUIRE(set_stream_cta_limit(stream, ctas) == 0, "set_stream_cta_limit: more than 16 capped streams");
   return 0;
 }
-// 1 (default) = GEMMs whose 128-wide tiling would occupy at most half of the SMs use 64-wide N tiles (twice the CTAs, half the serial work
-// per CTA); 0 = always the widest tile.  Scheduling only: results are unchanged.
-RIH_API int rih_set_narrow_tiles(int on) { tc::set_narrow_small(on); return 0; }
-// 1 (default) = convolution weight gradients with Cin % 32 == 0 use 256-wide N tiles that span several filter taps; 0 = one tap per tile.
-// Scheduling / tiling only: results agree up to the summation order of the split-K reduction.
-// 1 (default) = stride-2 convolutions (forward, weight gradient, input gradient) address the full-resolution tensors in place through tensor
-// maps with element strides {1, 2, 2, 1}; the input gradient runs as four dense parity-class GEMMs.  0 = the copy-based formulation
-// (parity-stacked input for forward / wgrad, zero-inserted dY for dgrad; needs the rih_conv2d_workspace buffers).
 // out[0..2] = tensor-core GEMM launches with the TMA-store epilogue, with per-thread stores, exact-fp32 SIMT GEMM launches since the last reset
 RIH_API int rih_gemm_launch_counts(long long* out, int reset) {
   if (out) for (int i = 0; i < 3; ++i) out[i] = tc::g_launch_counts[i];
@@ -72,11 +60,13 @@ RIH_API int rih_gemm_dgrad_t_launches(long long* out, int reset) {
   if (reset) tc::g_dgrad_t_launches = 0;
   return 0;
 }
-RIH_API int rih_set_tma_grouped(int on) { tc::set_tma_grouped(on); return 0; }
+// Epilogue options of the tensor-core GEMM (default 7): bit 0 = residual rows prefetched a chunk ahead, bit 1 = bias / folded BatchNorm column
+// vectors cached in shared memory, bit 2 = the producer warp issues a k-block's TMA boxes from all lanes.  Scheduling only: results are unchanged.
 RIH_API int rih_set_epilogue_opt(int bits) { tc::set_epilogue_opt(bits); return 0; }
-RIH_API int rih_set_tma_res(int on) { tc::set_tma_res(on); return 0; }
+// 1 (default) = stride-2 convolutions (forward, weight gradient, input gradient) address the full-resolution tensors in place through tensor
+// maps with element strides {1, 2, 2, 1}; the input gradient runs as four dense parity-class GEMMs.  0 = the copy-based formulation
+// (parity-stacked input for forward / wgrad, zero-inserted dY for dgrad; needs the rih_conv2d_workspace buffers).
 RIH_API int rih_set_s2_direct(int on) { tc::set_s2_direct(on); return 0; }
-RIH_API int rih_set_wgrad_wide(int on) { tc::set_wgrad_wide(on); return 0; }
 // Bit mask of the register-A main loops of the wgmma GEMM (default 3):
 //   bit 0: the 3x3 / strided convolution weight gradients and the stem's (rih_conv2d_wgrad, rih_stem_conv_wgrad) read their MN-major dY operand
 //          from shared memory into registers and multiply it with the register-A form of wgmma; only the input operand is transposed in shared memory.

@@ -168,9 +168,6 @@ struct Epilogue {
   double* stats;                               // optional [2*N] column sum / sum of squares of the stored values (fused BatchNorm statistics)
   int s2_w2, s2_h2, s2_ph, s2_pw;              // tensor-core stride-2 dgrad (s2_w2 > 0): the tile's 128 rows are pixels (n, i, j) of the half-resolution grid
                                                // s2_h2 x s2_w2; they are stored to input pixels (2 i + s2_ph, 2 j + s2_pw) through an element-strided 4-D map
-  int kb_rotate;                               // tensor-core persistent kernel: start each tile's k loop at a tile-dependent k-block and wrap around (rih_set_k_rotation)
-  int reverse;                                 // tensor-core persistent kernel: walk the output tiles from the last to the first (see rih_set_traversal)
-  unsigned long long a_policy;                 // tensor-core path: L2 eviction-priority policy for the A-operand TMA loads (0 = none)
   int nv_pad, nv_real;                         // tensor-core wgrad with Cin % BN != 0: column n of the (virtual) tile grid is (tap = n / nv_pad, c = n % nv_pad), stored iff c < nv_real
   const float* col_scale; const float* col_shift;   // optional per-column affine (an eval-mode BatchNorm folded into the producing convolution):
   int affine_post;                             //   0: applied to the accumulator BEFORE bias / ReLU (torchvision order Conv -> BN -> (+res) -> ReLU)
@@ -201,7 +198,7 @@ struct Epilogue {
 };
 static inline Epilogue make_epilogue(float* c, int ldc, int M, int N, const float* bias, int relu, int mode) {
   Epilogue e; e.c = c; e.ldc = ldc; e.M = M; e.N = N; e.bias = bias; e.relu = relu; e.mode = mode;
-  e.res = nullptr; e.ldres = 0; e.seed_ptr = nullptr; e.site = 0; e.thresh = 0; e.inv_keep = 1.f; e.stats = nullptr; e.scale = 1.f; e.nv_pad = 0; e.nv_real = 0; e.s2_w2 = 0; e.s2_h2 = 0; e.s2_ph = 0; e.s2_pw = 0; e.kb_rotate = 0; e.reverse = 0; e.a_policy = 0ull;
+  e.res = nullptr; e.ldres = 0; e.seed_ptr = nullptr; e.site = 0; e.thresh = 0; e.inv_keep = 1.f; e.stats = nullptr; e.scale = 1.f; e.nv_pad = 0; e.nv_real = 0; e.s2_w2 = 0; e.s2_h2 = 0; e.s2_ph = 0; e.s2_pw = 0;
   e.col_scale = nullptr; e.col_shift = nullptr; e.affine_post = 0; e.relu_post = 0; e.opt = 7;
   return e;
 }

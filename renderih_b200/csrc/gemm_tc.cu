@@ -137,37 +137,24 @@ int make_tmap_wgrad_out(CUtensorMap* map, const float* base, int Cout, int taps,
 }
 
 int g_stats_fused = 0;            // set by the launcher when the epilogue accumulated ep.stats (fused BatchNorm statistics)
-static int g_wgrad_wide = 3;     // multi-tap N tiles for the convolution weight gradients, also over padded channel counts (rih_set_wgrad_wide)
-void set_wgrad_wide(int on) { g_wgrad_wide = on & 3; }     // bit 0: multi-tap 128-wide tiles, bit 1: also for channel counts that are not multiples of 32
-static int g_narrow_small = 1;   // 64-wide N tiles for GEMMs whose 128-wide tiling would leave half of the SMs idle (RIH_NARROW_TILES=0 to compare)
-void set_narrow_small(int on) { g_narrow_small = on ? 1 : 0; }
-static int g_persistent = 1;     // 0 = one CTA per tile (non-persistent kernel; debug / comparison)
-void set_persistent(int on) { g_persistent = on ? 1 : 0; }
-static int g_tma_epilogue = 1;   // 0 = per-thread global stores (debug / comparison)
-void set_tma_epilogue(int on) { g_tma_epilogue = on ? 1 : 0; }
-long long g_launch_counts[3] = {0, 0, 0};
-long long g_dgrad_t_launches = 0;           // transposed-output (OUT_T) launches (rih_gemm_dgrad_t_launches)   // tensor-core launches with the TMA-store epilogue / with per-thread stores / SIMT GEMM launches (rih_gemm_launch_counts)
-static int g_tma_grouped = 7;    // grouped rank-3 tensor maps for MN-major operands (rih_set_tma_grouped)
-void set_tma_grouped(int on) { g_tma_grouped = on & 7; }       // bit 0: rank-3 grouped maps for dense MN-major operands / dY, bit 1: rank-5 grouped input maps of the conv wgrad, bit 2: grouped weight boxes of the conv dgrad
+long long g_launch_counts[3] = {0, 0, 0};   // tensor-core launches with the TMA-store epilogue / with per-thread stores / SIMT GEMM launches (rih_gemm_launch_counts)
+long long g_dgrad_t_launches = 0;           // transposed-output (OUT_T) launches (rih_gemm_dgrad_t_launches)
 static int g_epi_opt = 7;        // Epilogue::opt of every launch (rih_set_epilogue_opt)
 void set_epilogue_opt(int v) { g_epi_opt = v & 7; }
 static int g_gemm_rs = 3;        // register-A main loops (rih_set_gemm_rs): bit 0 = the 3x3 / strided convolution weight gradients and the stem's,
                                  // bit 1 = transposed-output input gradients (dgrad_t) and every other MN-major A operand
 void set_gemm_rs(int bits) { g_gemm_rs = bits & 3; }
-static int g_tma_res = 1;        // residual rows read by the TMA-store epilogue (0: GEMMs with a residual use per-thread global stores, as before)
-void set_tma_res(int on) { g_tma_res = on ? 1 : 0; }
 template <int BN, bool A_MN, bool B_MN, class Producer, int NSPLIT, bool A_RS, bool OUT_T>
 static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep, const Producer& prod, int M, int N, int num_kb, int splits,
                       int kb_per_split, cudaStream_t s, const CUtensorMap* c_map = nullptr) {
   // TMA-store epilogue whenever the output is a 16-byte aligned matrix (a residual is read back row-wise by the epilogue threads when it is aligned too)
   CUtensorMap tc_;
   int tma_epi = 0;
-  if (c_map) {       // caller-built output map (3-D wgrad view); only the persistent TMA-store epilogue understands it
-    if (!g_persistent) { set_error("gemm_tc: output-map override needs the persistent kernel"); return 1; }
+  if (c_map) {       // caller-built output map (3-D wgrad view)
     tc_ = *c_map;
     tma_epi = 1;
-  } else if ((!ep.res || (g_tma_res && splits == 1 && ((reinterpret_cast<uintptr_t>(ep.res) & 15) == 0) && ep.ldres % 4 == 0 && N % 4 == 0)) &&
-             ((reinterpret_cast<uintptr_t>(ep.c) & 15) == 0) && (ep.ldc % 4 == 0) && g_tma_epilogue) {
+  } else if ((!ep.res || (splits == 1 && ((reinterpret_cast<uintptr_t>(ep.res) & 15) == 0) && ep.ldres % 4 == 0 && N % 4 == 0)) &&
+             ((reinterpret_cast<uintptr_t>(ep.c) & 15) == 0) && (ep.ldc % 4 == 0)) {
     if (make_tmap_2d(&tc_, ep.c, M, N, ep.ldc, BM)) return 1;
     tma_epi = 1;
   } else {
@@ -192,14 +179,14 @@ static int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep,
   }
   const int tiles_n = cdiv(N, BN), tiles_m = cdiv(M, BM);
   const long long total = (long long)tiles_n * tiles_m * splits;
-  // persistent: at most one CTA per SM (fewer on a CTA-capped stream); otherwise one CTA per tile
-  const long long cap = g_persistent ? stream_cta_limit(s, sm_count()) : total;
+  // persistent: at most one CTA per SM (fewer on a CTA-capped stream)
+  const long long cap = stream_cta_limit(s, sm_count());
   const int ctas = (int)(total < cap ? total : cap);
-  if (ep.stats && !(g_persistent && tma_epi && splits == 1)) ep.stats = nullptr;
+  if (ep.stats && !(tma_epi && splits == 1)) ep.stats = nullptr;
   g_stats_fused = ep.stats != nullptr;
   launch_k(pk, dim3(ctas), dim3(persistent_threads<A_MN, B_MN, NSPLIT, A_RS>()), (size_t)smem_bytes<BN, NSPLIT>(), s, ta, tb, tc_, ep, prod, num_kb, kb_per_split,
            tiles_m, tiles_n, splits, tma_epi);
-  return check_launch(g_persistent ? "gemm_tc_persistent" : "gemm_tc");
+  return check_launch("gemm_tc_persistent");
 }
 static int g_nsplit = 1;   // set per call by the dispatchers below (1 = TF32, 2 = TF32 rn, 3 = 3xTF32)
 static float g_scale = 1.f; // accumulator scale (bias-compensated truncating TF32)
@@ -208,9 +195,6 @@ template <int BN, bool A_MN, bool B_MN, class Producer, bool A_RS = false, bool 
 static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, Epilogue ep, const Producer& prod, int M, int N, int num_kb, int splits,
                       int kb_per_split, cudaStream_t s, const CUtensorMap* c_map = nullptr) {
   ep.scale = g_scale;
-  ep.reverse = g_reverse;
-  ep.kb_rotate = g_kb_rotate;
-  ep.a_policy = g_l2_hints ? 1ull : 0ull;
   ep.opt = g_epi_opt;
   if (g_nsplit == 3) return launch_one<BN, A_MN, B_MN, Producer, 3, A_RS, OUT_T>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
   if (g_nsplit == 2) return launch_one<BN, A_MN, B_MN, Producer, 2, A_RS, OUT_T>(ta, tb, ep, prod, M, N, num_kb, splits, kb_per_split, s, c_map);
@@ -246,7 +230,7 @@ static void plan_splitk(Epilogue& ep, int M, int N, int BN, int num_kb, int allo
 // columns (input channels / in-features): narrower outputs would leave rows empty and keep the untransposed product (measured per shape:
 // tools/bench_dgrad.py).  The epilogue of the transposed form only scales and stores / accumulates into a 16-byte aligned output.
 static bool dgrad_t(const Epilogue& ep, int cols) {
-  return (g_gemm_rs & 2) && g_persistent && g_tma_epilogue && cols >= 128 &&
+  return (g_gemm_rs & 2) && cols >= 128 &&
          ep.mode <= 1 && !ep.bias && !ep.relu && !ep.res && !ep.stats && !ep.thresh && !ep.col_scale && !ep.relu_post &&
          (reinterpret_cast<uintptr_t>(ep.c) & 15) == 0 && ep.ldc % 4 == 0;
 }
@@ -254,7 +238,7 @@ static bool dgrad_t(const Epilogue& ep, int cols) {
 // c[M, N] (+)= a[M, K] . b[K, N] (a K-major, b MN-major) as c^T = b^T a^T: b is the MN-major A operand of a register-A, transposed-output launch
 static int gemm_tf32_t(const float* a, long long lda, const float* b, long long ldb, Epilogue ep, int M, int N, int K, cudaStream_t s) {
   CUtensorMap ta, tb, tcm;
-  const int a_grp = ((g_tma_grouped & 1) && N % 32 == 0) ? 1 : 0;
+  const int a_grp = N % 32 == 0 ? 1 : 0;
   if (a_grp ? make_tmap_2d_grouped(&ta, b, K, N, ldb, BM / 32) : make_tmap_2d(&ta, b, K, N, ldb, 32, true)) return 1;
   if (make_tmap_2d(&tb, a, M, K, lda, 128)) return 1;
   if (make_tmap_2d(&tcm, ep.c, M, N, ep.ldc, 128)) return 1;
@@ -269,13 +253,9 @@ int gemm_tf32(const float* a, long long lda, int a_mn, const float* b, long long
   if (M <= 0 || N <= 0) return 0;
   if (a_mn == 0 && b_mn == 1 && !allow_splitk && dgrad_t(ep, N)) return gemm_tf32_t(a, lda, b, ldb, ep, M, N, K, s);
   CUtensorMap ta, tb;
-  int BN = (N > 64) ? 128 : 64;
-  // Latency-bound GEMMs of the token decoder (a few dozen 128-row tiles, K <= 512): when 128-wide tiles would occupy at most half of the SMs,
-  // 64-wide tiles put twice as many CTAs to work -- each splits / multiplies half the B tile and drains half the accumulator, which is what a
-  // single-tile-per-CTA dependent chain (TMA -> split -> MMA -> epilogue) is made of.
-  if (BN == 128 && g_persistent && g_narrow_small && (long long)cdiv(M, BM) * cdiv(N, 128) <= sm_count() / 2) BN = 64;
-  // MN-major operands with a multiple of 32 columns: ONE grouped box per k-block instead of BM / 32 (BN / 32) four-KB boxes (rih_set_tma_grouped)
-  const int a_grp = (a_mn && (g_tma_grouped & 1) && M % 32 == 0) ? 1 : 0, b_grp = (b_mn && (g_tma_grouped & 1) && N % 32 == 0) ? 1 : 0;
+  const int BN = (N > 64) ? 128 : 64;
+  // MN-major operands with a multiple of 32 columns: ONE grouped box per k-block instead of BM / 32 (BN / 32) four-KB boxes
+  const int a_grp = (a_mn && M % 32 == 0) ? 1 : 0, b_grp = (b_mn && N % 32 == 0) ? 1 : 0;
   if (a_mn ? (a_grp ? make_tmap_2d_grouped(&ta, a, K, M, lda, BM / 32) : make_tmap_2d(&ta, a, K, M, lda, 32, true)) : make_tmap_2d(&ta, a, M, K, lda, BM)) return 1;
   if (b_mn ? (b_grp ? make_tmap_2d_grouped(&tb, b, K, N, ldb, BN / 32) : make_tmap_2d(&tb, b, K, N, ldb, 32, true)) : make_tmap_2d(&tb, b, N, K, ldb, BN)) return 1;
   int num_kb = cdiv(K, BK), splits, kps;
@@ -320,7 +300,7 @@ bool conv_tc_supported(const ConvGeom& g, int which /*0 fwd, 1 dgrad, 2 wgrad*/)
   if (which == 1 && g.stride == 2 && g_s2_direct)     // four parity-class GEMMs over the half-resolution (= output) grid
     return pow2(g.Wo) && pow2(g.Ho) && g.Wo <= 128 && ((long long)g.N * g.Ho * g.Wo) % BM == 0 && (g.Wo * g.Ho >= BM || BM % (g.Wo * g.Ho) == 0);
   if (which == 1) return pow2(g.W) && pow2(g.H) && g.W <= 128 && ((long long)g.N * g.H * g.W) % BM == 0 && (g.W * g.H >= BM || BM % (g.W * g.H) == 0);
-  return pow2(g.Wo) && pow2(g.Ho) && (g.Ho * g.Wo) % 32 == 0 && (g.Cin % 64 == 0 || g_persistent);
+  return pow2(g.Wo) && pow2(g.Ho) && (g.Ho * g.Wo) % 32 == 0;
 }
 
 long long conv_tc_workspace(const ConvGeom& g, int which) {
@@ -364,8 +344,8 @@ static int conv_dgrad_s2_direct(const float* dy, const float* w, Epilogue ep, co
   const int tile_n = BM / (W2 * tile_h);
   CUtensorMap ta, tb, tcm;
   if (make_tmap_nhwc(&ta, dy, g.N, g.Ho, g.Wo, g.Cout, g.ldy, W2, tile_h, tile_n, false)) return 1;
-  // weights [Cout][R*S*Cin] as the MN-major B operand: one grouped box per k-block when Cin % 32 == 0 (rih_set_tma_grouped bit 2)
-  const int b_grp = ((g_tma_grouped & 4) && g.Cin % 32 == 0) ? 1 : 0;
+  // weights [Cout][R*S*Cin] as the MN-major B operand: one grouped box per k-block when Cin % 32 == 0
+  const int b_grp = g.Cin % 32 == 0 ? 1 : 0;
   if (b_grp ? make_tmap_2d_grouped(&tb, w, g.Cout, (long long)g.R * g.S * g.Cin, (long long)g.R * g.S * g.Cin, BN / 32)
             : make_tmap_2d(&tb, w, g.Cout, (long long)g.R * g.S * g.Cin, (long long)g.R * g.S * g.Cin, 32, true)) return 1;
   if (make_tmap_nhwc(&tcm, ep.c, g.N, g.H, g.W, g.Cin, ep.ldc, W2, tile_h, tile_n, false, 2)) return 1;
@@ -435,8 +415,8 @@ int conv_dgrad_tf32(const float* dy, const float* w, Epilogue ep, const ConvGeom
   const int tile_n = BM / (g.W * tile_h);
   CUtensorMap ta, tb;
   if (make_tmap_nhwc(&ta, dy, g.N, g.Ho, g.Wo, g.Cout, g.ldy, g.W, tile_h, tile_n, false)) return 1;
-  // weights [Cout][R*S*Cin] as the MN-major B operand: one grouped box per k-block when Cin % 32 == 0 (rih_set_tma_grouped bit 2)
-  const int b_grp = ((g_tma_grouped & 4) && g.Cin % 32 == 0) ? 1 : 0;
+  // weights [Cout][R*S*Cin] as the MN-major B operand: one grouped box per k-block when Cin % 32 == 0
+  const int b_grp = g.Cin % 32 == 0 ? 1 : 0;
   if (b_grp ? make_tmap_2d_grouped(&tb, w, g.Cout, (long long)g.R * g.S * g.Cin, (long long)g.R * g.S * g.Cin, BN / 32)
             : make_tmap_2d(&tb, w, g.Cout, (long long)g.R * g.S * g.Cin, (long long)g.R * g.S * g.Cin, 32, true)) return 1;
   ConvTcGeom cg{g.Cin, g.Cout, g.R, g.S, g.pad, g.H, g.W, g.Ho, g.Wo, tile_h, 0, g.Cin};
@@ -481,24 +461,24 @@ int stem_wgrad_tf32(const float* dy, int lddy, const float* xp, Epilogue ep, int
 int conv_wgrad_tf32(const float* dy, const float* x, Epilogue ep, const ConvGeom& g, float* ws, cudaStream_t s) {
   const int P = g.N * g.Ho * g.Wo, taps = g.R * g.S, Nn = taps * g.Cin;
   // Cin a multiple of 32: the 32-column chunks of an N tile never straddle a tap, so 128-wide tiles may span several taps (Cin = 32, 64:
-  // the dY operand is re-read once per N tile instead of once per tap and channel block) -- RIH_WGRAD_WIDE=0 keeps one tap per tile
+  // the dY operand is re-read once per N tile instead of once per tap and channel block).
   // Channel counts that are not multiples of 32 (HRNet's 48, 80, 208 ...) take the wide tiles too, on a "virtual" grid of cin32 = ceil32(Cin)
-  // columns per tap (rih_set_wgrad_wide bit 1): 48-channel convolutions would otherwise run nine 64-wide tiles (dY re-read 9 times);
-  // five 128-wide tiles over 9 x 64 virtual columns instead.
+  // columns per tap: 48-channel convolutions would otherwise run nine 64-wide tiles (dY re-read 9 times); five 128-wide tiles over 9 x 64
+  // virtual columns instead.
   const int cin32 = cdiv(g.Cin, 32) * 32;
-  const bool wide_pad = (g_wgrad_wide & 2) && g.Cin % 32 != 0 && g.Cin % 4 == 0 && taps * cin32 >= 128;
-  const bool wide = g_wgrad_wide && g_persistent && (g.Cin % 32 == 0 || wide_pad) && Nn >= 128;
+  const bool wide_pad = g.Cin % 32 != 0 && g.Cin % 4 == 0 && taps * cin32 >= 128;
+  const bool wide = (g.Cin % 32 == 0 || wide_pad) && Nn >= 128;
   const int BN = wide ? 128 : ((g.Cin % 128 == 0) ? 128 : 64);
   // N tiles never straddle a tap: each tap owns ceil(Cin / BN) tiles; when BN does not divide Cin (48, 96, ...) the tile grid is
   // "virtual" (cin_pad columns per tap) and the epilogue stores through a 3-D map [Cout][taps][Cin] that clips at the tap's edge
   const int cin_pad = wide ? cin32 : cdiv(g.Cin, BN) * BN, Ngrid = taps * cin_pad;
   const int bw = g.Wo < 32 ? g.Wo : 32, bh = 32 / bw;
   CUtensorMap ta, tb, tcm;
-  const int a_grp = ((g_tma_grouped & 1) && g.Cout % 32 == 0) ? 1 : 0;
+  const int a_grp = g.Cout % 32 == 0 ? 1 : 0;
   if (a_grp ? make_tmap_2d_grouped(&ta, dy, P, g.Cout, g.ldy, BM / 32) : make_tmap_2d(&ta, dy, P, g.Cout, g.ldy, 32, true)) return 1;
-  // input chunks of one tap merged into grouped rank-5 boxes (rih_set_tma_grouped bit 1): b_grp = gcd(chunks per tap, 4) consecutive chunks per box
+  // input chunks of one tap merged into grouped rank-5 boxes: b_grp = gcd(chunks per tap, 4) consecutive chunks per box
   int b_grp = 0;
-  if ((g_tma_grouped & 2) && wide && !wide_pad && (g.stride == 1 || g_s2_direct)) {
+  if (wide && !wide_pad && (g.stride == 1 || g_s2_direct)) {
     const int per_tap = g.Cin / 32;
     b_grp = (per_tap % 4 == 0) ? 4 : ((per_tap % 2 == 0) ? 2 : 0);
   }
@@ -542,20 +522,8 @@ using namespace rih;
 RIH_API int rih_gemm_tf32(const float* a, long long lda, int a_mn, const float* b, long long ldb, int b_mn, float* c, int ldc,
                           int M, int N, int K, const float* bias, int relu, int accumulate, int allow_splitk, int nsplit, cudaStream_t stream) {
   RIH_REQUIRE(M >= 0 && N > 0 && K > 0, "gemm_tf32: bad shape");
-  // nsplit: 1 = TF32, 3 = 3xTF32.  Debug variants: negative = per-thread-store epilogue, +10 = non-persistent kernel, +20 = narrow tiles
-  // (accepted for compatibility: the tiles are at most 128 wide on every path).
-  int v = nsplit < 0 ? -nsplit : nsplit;
-  if (v >= 20) v -= 20;
-  const int nonpersistent = v >= 10;
-  if (nonpersistent) v -= 10;
-  RIH_REQUIRE(v == 1 || v == 2 || v == 3, "gemm_tf32: nsplit must be 1 (TF32, truncating), 2 (TF32, round-to-nearest) or 3 (3xTF32)");
-  tc::set_tma_epilogue(nsplit > 0);
-  tc::set_persistent(!nonpersistent);
-  nsplit = v;
+  RIH_REQUIRE(nsplit == 1 || nsplit == 2 || nsplit == 3, "gemm_tf32: nsplit must be 1 (TF32, truncating), 2 (TF32, round-to-nearest) or 3 (3xTF32)");
   tc::set_nsplit(nsplit);
   Epilogue ep = make_epilogue(c, ldc, M, N, bias, relu, accumulate ? 1 : 0);
-  int rc = tc::gemm_tf32(a, lda, a_mn, b, ldb, b_mn, ep, M, N, K, allow_splitk, stream);
-  tc::set_tma_epilogue(1);
-  tc::set_persistent(1);
-  return rc;
+  return tc::gemm_tf32(a, lda, a_mn, b, ldb, b_mn, ep, M, N, K, allow_splitk, stream);
 }

@@ -197,7 +197,7 @@ struct DenseProducer {
   // single-thread form (fully unrolled).  K-major operands are one box each and stay with lane 0 / lane 1.
   static constexpr bool WIDE_OK = A_MN || B_MN;
   int kbeg;
-  unsigned long long a_policy;   // L2 hint of the streamed activation operand (K-major A; K-major B = dY when A is MN-major, the transposed dgrad); 0 = no hint
+  unsigned long long a_policy;   // L2 evict-first policy of the streamed activation operand (K-major A; K-major B = dY when A is MN-major, the transposed dgrad)
   // a_grp / b_grp != 0: the MN-major operand comes through a "grouped" rank-3 tensor map {32 columns of a group, k rows, column groups} whose box
   // {32, 32, BM/32 or BN/32} lands in shared memory as the same [group][k row][32] chunks -- ONE TMA operation per operand and k-block
   // instead of one per 32-column chunk (make_tmap_2d_grouped; needs a column count that is a multiple of 32)
@@ -206,7 +206,7 @@ struct DenseProducer {
   template <bool W>
   __device__ __forceinline__ void load(const CUtensorMap* ta, const CUtensorMap* tb, int kb, int m0, int n0, int z, uint8_t* sa, uint8_t* sb, uint64_t* bar, int lane) const {
     const int k0 = kb * BK;
-    if constexpr (!A_MN) { if (!W || lane == 0) { if (a_policy) tma_load_2d_hint(sa, ta, k0, m0, bar, a_policy); else tma_load_2d(sa, ta, k0, m0, bar); } }
+    if constexpr (!A_MN) { if (!W || lane == 0) tma_load_2d_hint(sa, ta, k0, m0, bar, a_policy); }
     else if (a_grp) { if (!W || lane == 0) tma_load_3d(sa, ta, 0, k0, m0 >> 5, bar); }
     else if constexpr (W) { if (lane < BM / 32) tma_load_2d(sa + lane * (BK * 128), ta, m0 + lane * 32, k0, bar); }
     else {
@@ -214,7 +214,7 @@ struct DenseProducer {
       for (int c = 0; c < BM / 32; ++c) tma_load_2d(sa + c * (BK * 128), ta, m0 + c * 32, k0, bar);
     }
     if constexpr (!B_MN) {
-      if (!W || lane == BM / 32) { if (A_MN && a_policy) tma_load_2d_hint(sb, tb, k0, n0, bar, a_policy); else tma_load_2d(sb, tb, k0, n0, bar); }
+      if (!W || lane == BM / 32) { if (A_MN) tma_load_2d_hint(sb, tb, k0, n0, bar, a_policy); else tma_load_2d(sb, tb, k0, n0, bar); }
     }
     else if (b_grp) { if (!W || lane == BM / 32) tma_load_3d(sb, tb, 0, k0, n0 >> 5, bar); }
     else if constexpr (W) { const int c = lane - BM / 32; if (c >= 0 && c < BN / 32) tma_load_2d(sb + c * (BK * 128), tb, n0 + c * 32, k0, bar); }
@@ -264,7 +264,7 @@ struct ConvFwdProducer {
       s2_tap(r, g.pad, ph, dh);
       s2_tap(s, g.pad, pw, dw_);
       tma_load_4d(sa, ta, c0, dw_, oh0 + dh, (ph * 2 + pw) * g.s2_images + n, bar);
-    } else if (a_policy && g.R == 1) {
+    } else if (g.R == 1) {
       tma_load_4d_hint(sa, ta, c0, s - g.pad, oh0 + r - g.pad, n, bar, a_policy);    // single-tap only: a 3x3 re-reads every input tile nine times
     } else {
       tma_load_4d(sa, ta, c0, s - g.pad, oh0 + r - g.pad, n, bar);
@@ -607,8 +607,8 @@ template <int NSPLIT> __device__ __forceinline__ void split_frag(const uint32_t 
 }
 
 // ---------------------------------------------------------------- the kernel
-// Persistent: the grid is at most one CTA per SM and loops over output tiles (static round-robin); a grid of one CTA per tile is the
-// non-persistent form.  The shared-memory stage ring runs continuously across tiles, so the TMA loads of tile i+1 overlap the epilogue of tile i.
+// Persistent: the grid is at most one CTA per SM and loops over output tiles (static round-robin).  The shared-memory stage ring runs
+// continuously across tiles, so the TMA loads of tile i+1 overlap the epilogue of tile i.
 //   warpgroup 0: warp 0 = TMA producer (warps 1-3 idle)
 //   warpgroup 1 (only when an operand needs a transpose, rounding or a split in shared memory): operand preparation (prep_operand)
 //   last two warpgroups: consumers -- wgmma over rows [64 wg, 64 wg + 64) of the tile, then the epilogue of the chunks c with c % 2 == wg
@@ -621,8 +621,7 @@ template <int NSPLIT> __device__ __forceinline__ void split_frag(const uint32_t 
 // operand -- no operand is transposed in shared memory.  The accumulator is staged transposed (BM / 32 chunks of [BN rows x 128 B], one per
 // 32 output columns) and stored with tmap_c / ep over the [pixels x channels] output; only ep.scale and store / accumulate (mode 0 / 1) apply.
 // Tile order: the m tiles (channels) of one n tile (pixels) run on neighbouring CTAs, so a dY tile is fetched from HBM once and then hit in L2.
-// This numbers every output tile exactly as the untransposed product with 128-wide tiles does, so the k-block rotation (rih_set_k_rotation),
-// which starts a tile's k loop at (tile index) % (k-blocks), and the reverse traversal give both forms the same k order per output element.
+// Every tile runs its k-blocks in ascending order, so both forms accumulate each output element in the same k order.
 template <bool A_MN, bool B_MN, int NSPLIT, bool A_RS = false> __host__ __device__ constexpr bool has_prep() { return (A_MN && !A_RS) || B_MN || NSPLIT >= 2; }
 template <bool A_MN, bool B_MN, int NSPLIT, bool A_RS = false> __host__ __device__ constexpr int persistent_threads() { return (has_prep<A_MN, B_MN, NSPLIT, A_RS>() ? 4 : 3) * 128; }
 
@@ -663,7 +662,6 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
 
   // third tile coordinate z: split-K slice (kb_beg = z * kb_per_split)
   auto tile_coords = [&](int t, int& m0, int& n0, int& kb_beg, int& nkb, int& z) {
-    if (ep.reverse) t = total_tiles - 1 - t;          // serpentine traversal across consecutive kernels (rih_set_traversal)
     int mi, ni;
     if constexpr (OUT_T) {                            // the output's columns (m tiles) fastest, as for the untransposed product
       mi = t % tiles_m;
@@ -688,7 +686,7 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
     if (lane == 0 || wide_issue) {
       uint32_t it = 0;
       Producer pr = prod;
-      pr.set_policy(ep.a_policy ? l2_policy_evict_first() : 0ull);
+      pr.set_policy(l2_policy_evict_first());
       for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         int m0, n0, kb_beg, nkb, z;
         tile_coords(t, m0, n0, kb_beg, nkb, z);
@@ -701,15 +699,11 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
           }
           if (wide_issue) __syncwarp();
           uint8_t* sa = smem + s * STAGE_BYTES;
-          // k-block rotation: the sum over k does not care about the order, so each tile starts at its own k-block and wraps around --
-          // CTAs that run in lockstep then fetch DIFFERENT 128-byte slices of their (1 KB-pitch) rows at any instant
-          int kk = kb;
-          if (ep.kb_rotate) { kk = kb + (t % nkb); if (kk >= nkb) kk -= nkb; }
           if constexpr (Producer::WIDE_OK) {
-            if (wide_issue) pr.template load<true>(&tmap_a, &tmap_b, kb_beg + kk, m0, n0, z, sa, sa + A_BYTES, &full[s], lane);
-            else pr.template load<false>(&tmap_a, &tmap_b, kb_beg + kk, m0, n0, z, sa, sa + A_BYTES, &full[s], 0);
+            if (wide_issue) pr.template load<true>(&tmap_a, &tmap_b, kb_beg + kb, m0, n0, z, sa, sa + A_BYTES, &full[s], lane);
+            else pr.template load<false>(&tmap_a, &tmap_b, kb_beg + kb, m0, n0, z, sa, sa + A_BYTES, &full[s], 0);
           } else {
-            pr.template load<false>(&tmap_a, &tmap_b, kb_beg + kk, m0, n0, z, sa, sa + A_BYTES, &full[s], 0);
+            pr.template load<false>(&tmap_a, &tmap_b, kb_beg + kb, m0, n0, z, sa, sa + A_BYTES, &full[s], 0);
           }
         }
       }
@@ -768,7 +762,10 @@ gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
     float acc[BN / 2];
     RsFrag frag;
     if constexpr (A_RS) frag.init(wg, q, lane);
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    // the producer's tile walk, written with a tile counter: with `t += gridDim.x` ptxas spills more of the epilogue's registers
+    for (int i = 0; ; ++i) {
+      const int t = blockIdx.x + i * gridDim.x;
+      if (t >= total_tiles) break;
       int m0, n0, kb_beg, nkb, z;
       tile_coords(t, m0, n0, kb_beg, nkb, z);
       const int m = m0 + rr;

@@ -129,13 +129,9 @@ __global__ void bn_stats_kernel(const float* __restrict__ x, int ld, int M, int 
 // Thread -> (channel quad, first row) mapping shared by the element-wise BatchNorm passes: the launch has a multiple of C/4 threads, so
 // a thread keeps ONE channel quad for its whole grid-stride loop and the per-channel terms are computed once per thread.
 struct BnMap { int q; long long r0, rstride; };
-// HINT: streamed inputs of the element-wise BatchNorm passes are loaded with the evict-first priority (rih_set_l2_hints)
-// (compile-time switch: a run-time branch around every load kept the compiler from batching the loads of the unrolled row loop -- the
-// residual BatchNorm pass dropped from 5.8 to 4.6 TB/s)
-template <bool HINT> __device__ __forceinline__ float4 ld4(const float* p) {
-  if constexpr (HINT) return __ldcs(reinterpret_cast<const float4*>(p));
-  else return *reinterpret_cast<const float4*>(p);
-}
+// Streamed inputs of the element-wise BatchNorm passes are loaded with the evict-first priority, so that they do not displace the previous
+// kernel's output (which the next kernel is about to read) from the L2.
+__device__ __forceinline__ float4 ld4_stream(const float* p) { return __ldcs(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ BnMap bn_map(int C4) {
   const long long gid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   const long long T = (long long)gridDim.x * blockDim.x;
@@ -171,7 +167,6 @@ RIH_API int rih_bn_colstats(const float* x, int ld, int M, int C, double* ws, cu
 //                             unbiased variance, num_batches_tracked += 1 -- written once, by the threads that own row 0
 //   eval     (stats == NULL): from the running statistics
 // then y = (x - mean) * rstd * gamma + beta (+res) (relu).  mean / rstd are also stored for the backward pass.  C % 4 == 0, ld % 4 == 0.
-template <bool HINT>
 __global__ void __launch_bounds__(256)
 bn_forward_kernel(const float* __restrict__ x, int ldx, const double* __restrict__ stats, long long M, int C4, float eps, float momentum,
                   const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ res, int ldr,
@@ -206,12 +201,12 @@ bn_forward_kernel(const float* __restrict__ x, int ldx, const double* __restrict
   }
   const float4 g = *reinterpret_cast<const float4*>(gamma + c), b = *reinterpret_cast<const float4*>(beta + c);
   for (long long r = mp.r0; r < M; r += mp.rstride) {
-    const float4 v = ld4<HINT>(x + r * ldx + c);
+    const float4 v = ld4_stream(x + r * ldx + c);
     float4 o;
     o.x = (v.x - mu[0]) * rs[0] * g.x + b.x; o.y = (v.y - mu[1]) * rs[1] * g.y + b.y;
     o.z = (v.z - mu[2]) * rs[2] * g.z + b.z; o.w = (v.w - mu[3]) * rs[3] * g.w + b.w;
     if (res) {
-      const float4 q = ld4<HINT>(res + r * ldr + c);
+      const float4 q = ld4_stream(res + r * ldr + c);
       o.x += q.x; o.y += q.y; o.z += q.z; o.w += q.w;
     }
     if (relu) {
@@ -229,10 +224,8 @@ RIH_API int rih_bn_forward(const float* x, int ldx, const double* stats, long lo
                            float* mean_out, float* rstd_out, float* running_mean, float* running_var, long long* tracked, cudaStream_t s) {
   RIH_REQUIRE(C % 4 == 0 && ldx % 4 == 0 && ldy % 4 == 0 && (!res || ldr % 4 == 0), "bn_forward: needs C,ld %% 4 == 0");
   RIH_REQUIRE(M > 0 && (stats || (running_mean && running_var)), "bn_forward: eval mode needs the running statistics");
-  if (g_l2_hints) launch_k(bn_forward_kernel<true>, bn_grid(M, C / 4, 256, ew_ctas(s)), 256, 0, s, x, ldx, stats, M, C / 4, eps, momentum, gamma, beta, res, ldr, y, ldy, relu,
-                           relu_mask, mean_out, rstd_out, running_mean, running_var, tracked);
-  else launch_k(bn_forward_kernel<false>, bn_grid(M, C / 4, 256, ew_ctas(s)), 256, 0, s, x, ldx, stats, M, C / 4, eps, momentum, gamma, beta, res, ldr, y, ldy, relu,
-                relu_mask, mean_out, rstd_out, running_mean, running_var, tracked);
+  launch_k(bn_forward_kernel, bn_grid(M, C / 4, 256, ew_ctas(s)), 256, 0, s, x, ldx, stats, M, C / 4, eps, momentum, gamma, beta, res, ldr, y, ldy, relu,
+           relu_mask, mean_out, rstd_out, running_mean, running_var, tracked);
   return check_launch("bn_forward");
 }
 
@@ -285,7 +278,6 @@ bn_bwd_reduce_kernel(const float* __restrict__ dy, int lddy, const float* __rest
 }
 // backward pass 2 (the per-channel finalisation folded in): dx = gamma*rstd*(g - sum_g/M - xhat*sum_gx/M) [train] ; dres (+)= g ;
 // optional mask by (x>0) for Conv->ReLU->BN; the threads that own row 0 write dgamma / dbeta.  Same thread mapping as bn_forward_kernel.
-template <bool HINT>
 __global__ void __launch_bounds__(256)
 bn_bwd_apply_kernel(const float* __restrict__ dy, int lddy, const float* __restrict__ y, int ldy, const unsigned char* __restrict__ relu_mask,
                     const float* __restrict__ x, int ldx, const float* __restrict__ mean, const float* __restrict__ rstd,
@@ -314,9 +306,9 @@ bn_bwd_apply_kernel(const float* __restrict__ dy, int lddy, const float* __restr
     }
   }
   for (long long r = mp.r0; r < M; r += mp.rstride) {
-    const float4 g4 = ld4<HINT>(dy + r * lddy + c);
+    const float4 g4 = ld4_stream(dy + r * lddy + c);
     float g[4] = {g4.x, g4.y, g4.z, g4.w};
-    const float4 x4 = ld4<HINT>(x + r * ldx + c);
+    const float4 x4 = ld4_stream(x + r * ldx + c);
     const float xv[4] = {x4.x, x4.y, x4.z, x4.w};
     if (relu && relu_mask) {
       const unsigned m4 = relu_mask[r * C4 + mp.q];
@@ -372,10 +364,8 @@ RIH_API int rih_bn_bwd(const float* dy, int lddy, const float* y, int ldy, const
   dim3 grid(gx, cdiv(M, rows_per_cta));
   launch_k(bn_bwd_reduce_kernel, grid, 256, 0, s, dy, lddy, y, ldy, relu_mask, x, ldx, mean, rstd, gamma, beta, (int)M, C, rows_per_cta, relu, ws);
   if (int e = check_launch("bn_bwd_reduce")) return e;
-  if (g_l2_hints) launch_k(bn_bwd_apply_kernel<true>, bn_grid(M, C / 4, 256, ew_ctas(s)), 256, 0, s, dy, lddy, y, ldy, relu_mask, x, ldx, mean, rstd, gamma, beta, ws, dx, lddx,
-                           dres, lddr, dres_acc, dgamma, dbeta, param_acc, M, C / 4, relu, training, mask_input);
-  else launch_k(bn_bwd_apply_kernel<false>, bn_grid(M, C / 4, 256, ew_ctas(s)), 256, 0, s, dy, lddy, y, ldy, relu_mask, x, ldx, mean, rstd, gamma, beta, ws, dx, lddx,
-                dres, lddr, dres_acc, dgamma, dbeta, param_acc, M, C / 4, relu, training, mask_input);
+  launch_k(bn_bwd_apply_kernel, bn_grid(M, C / 4, 256, ew_ctas(s)), 256, 0, s, dy, lddy, y, ldy, relu_mask, x, ldx, mean, rstd, gamma, beta, ws, dx, lddx,
+           dres, lddr, dres_acc, dgamma, dbeta, param_acc, M, C / 4, relu, training, mask_input);
   return check_launch("bn_bwd_apply");
 }
 

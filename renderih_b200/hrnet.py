@@ -54,7 +54,7 @@ def conv_bn(x, conv, bn, N, H, training, relu=True, res=None, alias_input=False)
     route the residual use of x through x_alias and its gradient is accumulated by this convolution's dgrad kernel (ops.conv2d).
     Training-mode batch statistics come out of the convolution's epilogue when it runs on the tensor-core path."""
     k, st, pd = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-    fold = None if (training or alias_input or torch.is_grad_enabled() or conv.bias is not None or not ops.BN_FOLD) else bn.__dict__.get('_rih_fold')
+    fold = None if (training or alias_input or torch.is_grad_enabled() or conv.bias is not None) else bn.__dict__.get('_rih_fold')
     if fold is not None:       # inference: BatchNorm (+ residual + ReLU) in the convolution's epilogue (ops.conv2d_bn_eval)
         return ops.conv2d_bn_eval(x, conv.weight, N, H, H, st, pd, fold, order=0, relu=relu, res=res), (H + 2 * pd - k) // st + 1
     stats = torch.empty(2 * conv.out_channels, device=x.device, dtype=torch.float64) if training else None

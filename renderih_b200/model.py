@@ -56,7 +56,7 @@ def _conv_bn(x, conv, bn, N, H, W, training, relu=True, res=None, alias_input=Fa
     """torchvision order Conv -> BN -> (+res) -> ReLU.  alias_input: returns (y, Ho, x_alias) -- see ops.conv2d."""
     k = conv.kernel_size[0]
     fold = None if (training or alias_input or torch.is_grad_enabled() or conv.bias is not None) else bn.__dict__.get('_rih_fold')
-    if fold is not None and ops.BN_FOLD:     # inference: the BatchNorm (+ residual + ReLU) rides in the convolution's epilogue
+    if fold is not None:     # inference: the BatchNorm (+ residual + ReLU) rides in the convolution's epilogue
         y = ops.conv2d_bn_eval(x, conv.weight, N, H, W, conv.stride[0], conv.padding[0], fold, order=0, relu=relu, res=res)
         return y, (H + 2 * conv.padding[0] - k) // conv.stride[0] + 1
     stats = torch.empty(2 * conv.out_channels, device=x.device, dtype=torch.float64) if training else None
@@ -73,7 +73,7 @@ def _conv_bn(x, conv, bn, N, H, W, training, relu=True, res=None, alias_input=Fa
 def _conv_relu_bn(x, conv, bn, N, H, W, training):
     """repo order Conv -> ReLU -> BN (models/model_zoo/__init__.py:56-82, models/encoder.py:52-54)"""
     fold = None if (training or torch.is_grad_enabled() or conv.bias is not None) else bn.__dict__.get('_rih_fold')
-    if fold is not None and ops.BN_FOLD:
+    if fold is not None:
         return ops.conv2d_bn_eval(x, conv.weight, N, H, W, conv.stride[0], conv.padding[0], fold, order=1, relu=True)
     stats = torch.empty(2 * conv.out_channels, device=x.device, dtype=torch.float64) if training else None
     y = ops.conv2d(x, conv.weight, None, N, H, W, stride=conv.stride[0], pad=conv.padding[0], relu=True,
@@ -218,7 +218,7 @@ class ResNetSimple(nn.Module):
         if not img.requires_grad and ops.stem_supported(H, W):
             # conv1 straight from the NCHW image: zero-bordered NHWC4 copy + wgmma implicit GEMM (no im2col buffer), train and eval mode
             conv, bn = r.conv1, r.bn1
-            fold = None if (self.training or torch.is_grad_enabled() or not ops.BN_FOLD) else bn.__dict__.get('_rih_fold')
+            fold = None if (self.training or torch.is_grad_enabled()) else bn.__dict__.get('_rih_fold')
             stats = torch.empty(2 * 64, device=img.device, dtype=torch.float64) if self.training else None
             x = ops.stem_conv(img, conv.weight, stats, fold)
             if fold is None:

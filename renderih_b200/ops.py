@@ -16,8 +16,7 @@ call = _lib.call
 
 GROUP_FLOPS = {}      # entry point -> f(args) = algorithmic flops of one call (measurement metadata for bench.py's class roofline)
 GEMM_MODES = {'simt': 0, 'tf32': 1, 'tf32x3': 2, 'tf32rn': 3, 'tf32c': 4}
-import os as _os
-_ATTN = {'nsplit': 0, 'force': _os.environ.get('RIH_ATTN_IMPL') or None}     # RIH_ATTN_IMPL=simt|tc overrides the mode-derived choice (A/B runs)
+_ATTN = {'nsplit': 0}
 
 
 MODE = {'conv': 'simt', 'linear': 'simt'}
@@ -100,8 +99,8 @@ def _gt(t):
 # flat gradient buffer it is issued on a side stream that forks off the stream running backward, so the (latency-bound) chain
 # dgrad -> previous layer's backward does not wait for it.  All side streams are joined into the caller's stream by an autograd-engine
 # final callback when the backward pass ends (under CUDA-graph capture the fork / join become parallel graph branches).
-# RIH_WGRAD_STREAM=0 disables it.
-_WG = {'streams': {}, 'armed': False, 'enabled': _os.environ.get('RIH_WGRAD_STREAM', '1') != '0'}
+# _WG['enabled'] = False keeps them on the backward stream.
+_WG = {'streams': {}, 'armed': False, 'enabled': True}
 
 
 def _wgrad_fork(*tensors):
@@ -466,7 +465,6 @@ def attention(q, k, v, B, H, Sq, Sk, p_drop=0.0, impl=None):
     """impl: None = follow set_gemm_mode (SIMT fused kernel in 'simt' mode, tensor-core fused kernels otherwise), 'simt' | 'tc' to force."""
     site = seed_state.next_site() if p_drop > 0 else 0
     nsplit = _ATTN['nsplit']
-    impl = impl or _ATTN.get('force')
     if impl == 'simt':
         nsplit = 0
     elif impl == 'tc' and nsplit == 0:
@@ -656,8 +654,8 @@ class AttnProjFn(Function):
         return (dxq, dxkv, gw[0], gw[1], gw[2], gb[0], gb[1], gb[2]) + (None,) * 7
 
 
-FUSED = {'qkv': _os.environ.get('RIH_FUSED_QKV', '1') != '0',        # A/B switches: 0 = separate projection GEMMs + attention node
-         'alias': _os.environ.get('RIH_RES_ALIAS', '1') != '0'}       #               0 = residual-branch gradients summed by autograd adds
+FUSED = {'qkv': True,        # False = separate projection GEMMs + attention node
+         'alias': True}      # False = residual-branch gradients summed by autograd adds
 
 
 def attention_proj(xq, xkv, lin_q, lin_k, lin_v, B, H, Sq, Sk, p_drop=0.0):
@@ -671,11 +669,6 @@ def attention_proj(xq, xkv, lin_q, lin_k, lin_v, B, H, Sq, Sk, p_drop=0.0):
         return attention(q, k, v, B, H, Sq, Sk, p_drop=p_drop)
     site = seed_state.next_site() if p_drop > 0 else 0
     nsplit = _ATTN['nsplit']
-    impl = _ATTN.get('force')
-    if impl == 'simt':
-        nsplit = 0
-    elif impl == 'tc' and nsplit == 0:
-        nsplit = 3
     HD = lin_q.weight.shape[0]
     d = HD // H
     if not (nsplit and d % 4 == 0 and B * H > 0 and Sq > 0 and Sk <= 512):
@@ -915,8 +908,6 @@ def conv2d(x, w, b, N, H, W, stride=1, pad=0, relu=False, relu_masked_by_consume
 
 
 # ----------------------------------------------------------------------------- eval-mode BatchNorm folded into the convolution
-BN_FOLD = _os.environ.get('RIH_BN_FOLD', '1') != '0'
-
 
 class BnFold:
     """Per-channel (scale, shift) vectors of every eval-mode BatchNorm2d under `root`, recomputed by ONE kernel launch per forward pass from
@@ -968,7 +959,7 @@ class BnFold:
 
 def bn_fold_refresh(root):
     """Recompute the folded BatchNorm vectors of `root` (cached BnFold) when the folded inference path applies; returns True when it does."""
-    if not BN_FOLD or torch.is_grad_enabled():
+    if torch.is_grad_enabled():
         return False
     f = root.__dict__.get('_rih_bn_fold')
     if f is None:
@@ -1071,7 +1062,7 @@ class StemConvFn(Function):
 
 def stem_supported(H, W):
     """The implicit-GEMM stem needs a tensor-core convolution mode and 256 x 256 images (one output row = one 128-pixel tile)."""
-    return MODE['conv'] != 'simt' and H == W == 256 and _os.environ.get('RIH_STEM_IGEMM', '1') != '0'
+    return MODE['conv'] != 'simt' and H == W == 256
 
 
 def stem_conv(img, weight, stats=None, fold=None):

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """The convolution side of the step in isolation: ResNet-50 trunk (stem + layer1..4, train-mode BatchNorm) forward + backward at batch 64,
-captured into a CUDA graph and replayed -- the serial, bandwidth-bound 55 % of the training step (tools/timeline.py).  Used to A/B scheduling /
-tuning variants (RIH_LIB_VARIANT, RIH_SERPENTINE, RIH_L2_HINTS, RIH_PDL, ...) in one gpurun call, one process per variant:
+captured into a CUDA graph and replayed -- the serial, bandwidth-bound 55 % of the training step (tools/timeline.py).  Used to A/B the
+environment switches that remain (RIH_PDL), one process per variant:
 
-    RIH_SERPENTINE=1 python tools/trunk_bench.py  ->  one JSON line {variant flags, ms fwd, ms fwd+bwd}
+    RIH_PDL=1 python tools/trunk_bench.py  ->  one JSON line {variant flags, ms fwd, ms fwd+bwd}
 """
 import json
 import os
