@@ -75,6 +75,19 @@ __device__ __forceinline__ double warp_sum_d(double v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// Sum of v over a block of NW warps, returned to every thread: each warp's shuffle sum, then the warps' partials in warp order.
+// s_red holds NW floats; the leading barrier lets consecutive calls reuse it.
+template <int NW>
+__device__ __forceinline__ float block_sum(float v, float* s_red, int tid) {
+  v = warp_sum(v);
+  __syncthreads();
+  if ((tid & 31) == 0) s_red[tid >> 5] = v;
+  __syncthreads();
+  float t = 0.f;
+#pragma unroll
+  for (int i = 0; i < NW; ++i) t += s_red[i];
+  return t;
+}
 
 // i = q * d + r with a 32-bit fast path (64-bit integer division costs ~100 instructions and dominated the elementwise kernels)
 __device__ __forceinline__ void divmod(long long i, int d, bool small, long long& q, int& r) {

@@ -34,17 +34,6 @@ struct GeoConsts {
   const float* conv;      // [2,15,18] per hand and joint 1..15: P (row-major 3x3) then C
 };
 
-__device__ __forceinline__ float block_sum(float v, float* s_red, int tid) {
-  v = warp_sum(v);
-  __syncthreads();
-  if ((tid & 31) == 0) s_red[tid >> 5] = v;
-  __syncthreads();
-  float t = 0.f;
-#pragma unroll
-  for (int i = 0; i < NWARPS; ++i) t += s_red[i];
-  return t;
-}
-
 // anchorutils.py:57-64, with the reference's operation order (no contraction into FMAs)
 __device__ __forceinline__ void anchor_pos(const float* vb, const int* f, const float* w, float* out) {
   for (int c = 0; c < 3; ++c) {
@@ -192,9 +181,9 @@ geo_prior_fwd_kernel(GeoConsts gc, int A, int E, int D, const float* __restrict_
     mk += mask[base + o];
   }
   float out[5];
-  out[0] = block_sum(qn[0], s.red, tid); out[1] = block_sum(qn[1], s.red, tid);
-  out[2] = block_sum(ed[0], s.red, tid); out[3] = block_sum(ed[1], s.red, tid);
-  out[4] = block_sum(cn, s.red, tid);
+  out[0] = block_sum<NWARPS>(qn[0], s.red, tid); out[1] = block_sum<NWARPS>(qn[1], s.red, tid);
+  out[2] = block_sum<NWARPS>(ed[0], s.red, tid); out[3] = block_sum<NWARPS>(ed[1], s.red, tid);
+  out[4] = block_sum<NWARPS>(cn, s.red, tid);
   // integer mask count: a warp-shuffle sum of 64-bit partials, then the warps in order
   __shared__ long long s_mk[NWARPS];
   for (int o = 16; o > 0; o >>= 1) mk += __shfl_xor_sync(0xffffffffu, mk, o);
@@ -225,7 +214,7 @@ geo_prior_reduce_kernel(const float* __restrict__ part, const long long* __restr
     mk += count[b];
   }
   float S[7];
-  for (int k = 0; k < 7; ++k) S[k] = block_sum(acc[k], s_red, tid);
+  for (int k = 0; k < 7; ++k) S[k] = block_sum<NWARPS>(acc[k], s_red, tid);
   for (int o = 16; o > 0; o >>= 1) mk += __shfl_xor_sync(0xffffffffu, mk, o);
   if ((tid & 31) == 0) s_mk[tid >> 5] = mk;
   __syncthreads();
@@ -240,21 +229,6 @@ geo_prior_reduce_kernel(const float* __restrict__ part, const long long* __restr
     out[3] = S[5] / (float)B + S[6] / (float)B;
     *den_out = den;
   }
-}
-
-// R = M(p) / n with n = |p|^2  ->  dL/dp   (the quaternion chain of rih_manopth_bwd)
-__device__ void quat_R_backward(const float* p, const float* g, float* d) {
-  const float w = p[0], x = p[1], y = p[2], z = p[3];
-  const float n = w * w + x * x + y * y + z * z;
-  float R[9];
-  quat_to_R(w, x, y, z, R);
-  float gRR = 0.f;
-  for (int e = 0; e < 9; ++e) gRR += g[e] * R[e];
-  const float dw = 2.f * (w * (g[0] + g[4] + g[8]) + z * (g[3] - g[1]) + y * (g[2] - g[6]) + x * (g[7] - g[5]));
-  const float dx = 2.f * (x * (g[0] - g[4] - g[8]) + y * (g[1] + g[3]) + z * (g[2] + g[6]) + w * (g[7] - g[5]));
-  const float dy = 2.f * (y * (-g[0] + g[4] - g[8]) + x * (g[1] + g[3]) + z * (g[5] + g[7]) + w * (g[2] - g[6]));
-  const float dz = 2.f * (z * (-g[0] - g[4] + g[8]) + x * (g[2] + g[6]) + y * (g[5] + g[7]) + w * (g[3] - g[1]));
-  d[0] = (dw - 2.f * w * gRR) / n; d[1] = (dx - 2.f * x * gRR) / n; d[2] = (dy - 2.f * y * gRR) / n; d[3] = (dz - 2.f * z * gRR) / n;
 }
 
 __global__ void __launch_bounds__(THREADS)
@@ -327,8 +301,9 @@ geo_prior_bwd_kernel(GeoConsts gc, int A, int E, int D, int B, const float* __re
         const float nrm = sqrtf(n2), den_q = fmaxf(nrm, 1e-12f);
         const float sg = h ? -1.f : 1.f;
         const float p[4] = {q[0] / den_q, q[1] / den_q, sg * (q[2] / den_q), sg * (q[3] / den_q)};
-        float dp[4];
-        quat_R_backward(p, dR, dp);
+        float R[9], dp[4];
+        quat_to_R(p[0], p[1], p[2], p[3], R);
+        quat_R_backward(p, R, dR, dp);
         dp[2] *= sg; dp[3] *= sg;
         // q / max(|q|, eps): dq = dp / c - q (q . dp) / (|q| c^2) where |q| >= eps
         const float qdp = q[0] * dp[0] + q[1] * dp[1] + q[2] * dp[2] + q[3] * dp[3];

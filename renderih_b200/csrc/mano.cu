@@ -1,52 +1,33 @@
 // MANO forward kinematics + linear blend skinning as ONE kernel (one CTA per hand).
 // reference: ManoLayer.forward  models/manolayer.py:250-322 ; rodrigues_batch :32-48 ; pca2axis :163-166
-// Stage plan inside the CTA (warp roles):
-//   S1  all warps : PCA->axis-angle (45 dots), shape blend v_shaped = T + S*beta (2334 outputs, coalesced [10][2334] table)
-//   S2  warps 0   : Rodrigues x15 ; warps 1.. : joint regression j_tpose = Jreg @ v_shaped (warp per joint row)
+// Stage plan inside the CTA (warp roles); S1-S4 are mano_core.cuh's:
+//   S0  all warps : betas, root matrix, PCA->axis-angle (45 dots) or the 15 rotation matrices
+//   S1  all warps : shape blend v_shaped = T + S*beta (2334 outputs, coalesced [10][2334] table)
+//   S2  warp 0    : Rodrigues x15, vec(R - I) ; warps 1.. : joint regression j_tpose = Jreg @ v_shaped (warp per joint row)
 //   S3  warp 0    : serial FK chain over the kinematic tree ; warps 1.. : pose blend v_tpose += P*(R-I) ([135][2334] table)
 //   S4  all warps : LBS per vertex (16 joint weights as 4x float4), results kept in shared memory
-//   S5  warp 0    : joints (FK joints + 5 finger tips), reorder, centre
+//   S5  21 threads: joints (FK joints + 5 finger tips), reorder, centre
 //   S6  all warps : centre / scale / trans, coalesced stores
 #include "common.cuh"
+#include "mano_core.cuh"
 using namespace rih;
 
 struct ManoConsts {
   const float* comps;       // [45,45]  hands_components
   const float* hands_mean;  // [45]
-  const float* shapedirsT;  // [10][2334]
-  const float* posedirsT;   // [135][2334]
-  const float* v_template;  // [2334]
-  const float* jreg;        // [16,778]
-  const float* weights;     // [778,16]
+  ManoTables t;             // shapedirsT, posedirsT, v_template, jreg, weights
   int parent[16];
   int new_order[21];
   int tips[5];
 };
 
-constexpr int MANO_V = 778, MANO_V3 = 2334, MANO_THREADS = 512;
-
-__global__ void __launch_bounds__(MANO_THREADS)
-mano_fwd_kernel(ManoConsts mc, const float* __restrict__ root_rot, const float* __restrict__ pose, int use_pca, int ncomps,
-                const float* __restrict__ shape, const float* __restrict__ trans, const float* __restrict__ scale,
-                int center_idx, int new_skel, float* __restrict__ v_out, float* __restrict__ j_out) {
-  pdl_sync();
-  __shared__ float s_v[MANO_V3];        // v_shaped -> v_tpose -> v_output
-  __shared__ float s_axis[48];
-  __shared__ float s_R[16][9];          // [0] = root, [1..15] = pose rotations
-  __shared__ float s_ps[136];           // vec(R - I)
-  __shared__ float s_beta[10];
-  __shared__ float s_j[16][3];          // j_tpose
-  __shared__ float s_T[16][12];         // global SE3 (top 3 rows)
-  __shared__ float s_jo[21][3];         // joints before reorder
-  __shared__ float s_jf[21][3];         // final joints
-  __shared__ float s_center[3];
-  const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nwarps = MANO_THREADS / 32;
-
-  if (tid < 10) s_beta[tid] = shape[(size_t)b * 10 + tid];
-  if (tid < 9) s_R[0][tid] = root_rot[(size_t)b * 9 + tid];
-  __syncthreads();
-  // ---- S1
+// S0-S5, shared by both kernels: vl receives the skinned vertices (it may be f.vt), jf the joints in output order and center the
+// centre joint (0 when center_idx < 0), all before centre / scale / trans.  Ends with a __syncthreads().
+__device__ __forceinline__ void mano_forward(ManoState& f, float* s_axis, float* vl, float (*jf)[3], float* center, const ManoConsts& mc,
+                                             const float* __restrict__ root_rot, const float* __restrict__ pose, int use_pca, int ncomps,
+                                             const float* __restrict__ shape, int center_idx, int b, int tid) {
+  if (tid < 10) f.beta[tid] = shape[(size_t)b * 10 + tid];
+  if (tid < 9) f.R[0][tid] = root_rot[(size_t)b * 9 + tid];
   if (use_pca) {
     if (tid < 45) {
       float acc = 0.f;
@@ -54,129 +35,56 @@ mano_fwd_kernel(ManoConsts mc, const float* __restrict__ root_rot, const float* 
       s_axis[tid] = acc + mc.hands_mean[tid];
     }
   } else {
-    if (tid < 135) s_R[1 + tid / 9][tid % 9] = pose[(size_t)b * 135 + tid];
-  }
-  for (int o = tid; o < MANO_V3; o += MANO_THREADS) {
-    float acc = 0.f;
-#pragma unroll
-    for (int i = 0; i < 10; ++i) acc = fmaf(mc.shapedirsT[i * MANO_V3 + o], s_beta[i], acc);
-    s_v[o] = mc.v_template[o] + acc;
+    if (tid < 135) f.R[1 + tid / 9][tid % 9] = pose[(size_t)b * 135 + tid];
   }
   __syncthreads();
-  // ---- S2
-  if (warp == 0) {
+  mano_forward_state(f, mc.t, mc.parent, tid, [&](int lane) {
     if (use_pca && lane < 15) {
       float ax = s_axis[lane * 3], ay = s_axis[lane * 3 + 1], az = s_axis[lane * 3 + 2];
       float angle = sqrtf(ax * ax + ay * ay + az * az) + 1e-8f;   // manolayer.py:37 (eps added after the norm)
       float x = ax / angle, y = ay / angle, z = az / angle;
       float sn = sinf(angle), cs = cosf(angle), oc = 1.f - cs;
       // L = [[0,-z,y],[z,0,-x],[-y,x,0]] ; R = I + sin*L + (1-cos)*L@L
-      float* R = s_R[1 + lane];
+      float* R = f.R[1 + lane];
       R[0] = 1.f + oc * (-(z * z) - (y * y)); R[1] = -sn * z + oc * (x * y);        R[2] = sn * y + oc * (x * z);
       R[3] = sn * z + oc * (x * y);         R[4] = 1.f + oc * (-(z * z) - (x * x)); R[5] = -sn * x + oc * (y * z);
       R[6] = -sn * y + oc * (x * z);        R[7] = sn * x + oc * (y * z);           R[8] = 1.f + oc * (-(y * y) - (x * x));
     }
-  } else {
-    for (int o = warp - 1; o < 48; o += nwarps - 1) {
-      int jt = o / 3, c = o % 3;
-      float acc = 0.f;
-      for (int vtx = lane; vtx < MANO_V; vtx += 32) acc = fmaf(mc.jreg[jt * MANO_V + vtx], s_v[vtx * 3 + c], acc);
-      acc = warp_sum(acc);
-      if (lane == 0) s_j[jt][c] = acc;
-    }
-  }
-  __syncthreads();
-  if (tid < 135) { int k = tid % 9; s_ps[tid] = s_R[1 + tid / 9][k] - ((k == 0 || k == 4 || k == 8) ? 1.f : 0.f); }
-  __syncthreads();
-  // ---- S3
-  if (warp == 0) {
-    if (lane == 0) {
-      // local transform i: R_i, t_i = (I - R_i) j_i ; global = global[parent] o local  (manolayer.py:274-283)
-      for (int i = 0; i < 16; ++i) {
-        const float* R = s_R[i];
-        float jx = s_j[i][0], jy = s_j[i][1], jz = s_j[i][2];
-        float t[3];
-        t[0] = (1.f - R[0]) * jx + (-R[1]) * jy + (-R[2]) * jz;
-        t[1] = (-R[3]) * jx + (1.f - R[4]) * jy + (-R[5]) * jz;
-        t[2] = (-R[6]) * jx + (-R[7]) * jy + (1.f - R[8]) * jz;
-        if (i == 0) {
-          for (int r = 0; r < 3; ++r) { s_T[0][r * 4 + 0] = R[r * 3]; s_T[0][r * 4 + 1] = R[r * 3 + 1]; s_T[0][r * 4 + 2] = R[r * 3 + 2]; s_T[0][r * 4 + 3] = t[r]; }
-        } else {
-          const float* P = s_T[mc.parent[i]];
-          for (int r = 0; r < 3; ++r) {
-            float p0 = P[r * 4], p1 = P[r * 4 + 1], p2 = P[r * 4 + 2], p3 = P[r * 4 + 3];
-            s_T[i][r * 4 + 0] = p0 * R[0] + p1 * R[3] + p2 * R[6];
-            s_T[i][r * 4 + 1] = p0 * R[1] + p1 * R[4] + p2 * R[7];
-            s_T[i][r * 4 + 2] = p0 * R[2] + p1 * R[5] + p2 * R[8];
-            s_T[i][r * 4 + 3] = p0 * t[0] + p1 * t[1] + p2 * t[2] + p3;
-          }
-        }
-      }
-    }
-  } else {
-    for (int o = tid - 32; o < MANO_V3; o += MANO_THREADS - 32) {
-      float acc = 0.f;
-#pragma unroll 9
-      for (int i = 0; i < 135; ++i) acc = fmaf(mc.posedirsT[i * MANO_V3 + o], s_ps[i], acc);
-      s_v[o] += acc;
-    }
-  }
-  __syncthreads();
-  // ---- S4: LBS
-  for (int vtx = tid; vtx < MANO_V; vtx += MANO_THREADS) {
-    const float4* w4 = reinterpret_cast<const float4*>(mc.weights + (size_t)vtx * 16);
-    float w[16];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { float4 t = __ldg(w4 + i); w[4 * i] = t.x; w[4 * i + 1] = t.y; w[4 * i + 2] = t.z; w[4 * i + 3] = t.w; }
-    float T[12];
-#pragma unroll
-    for (int e = 0; e < 12; ++e) T[e] = 0.f;
-#pragma unroll
-    for (int jt = 0; jt < 16; ++jt)
-#pragma unroll
-      for (int e = 0; e < 12; ++e) T[e] = fmaf(w[jt], s_T[jt][e], T[e]);
-    float x = s_v[vtx * 3], y = s_v[vtx * 3 + 1], z = s_v[vtx * 3 + 2];
-    float ox = T[0] * x + T[1] * y + T[2] * z + T[3];
-    float oy = T[4] * x + T[5] * y + T[6] * z + T[7];
-    float oz = T[8] * x + T[9] * y + T[10] * z + T[11];
-    s_v[vtx * 3] = ox; s_v[vtx * 3 + 1] = oy; s_v[vtx * 3 + 2] = oz;   // own element only: no hazard
-  }
-  __syncthreads();
-  // ---- S5: joints
-  if (tid < 21) {
-    float jx, jy, jz;
-    if (tid == 0) { jx = s_j[0][0]; jy = s_j[0][1]; jz = s_j[0][2]; }
-    else if (tid < 16) {
-      const float* P = s_T[mc.parent[tid]];
-      float x = s_j[tid][0], y = s_j[tid][1], z = s_j[tid][2];
-      jx = P[0] * x + P[1] * y + P[2] * z + P[3];
-      jy = P[4] * x + P[5] * y + P[6] * z + P[7];
-      jz = P[8] * x + P[9] * y + P[10] * z + P[11];
-    } else {
-      int vtx = mc.tips[tid - 16];
-      jx = s_v[vtx * 3]; jy = s_v[vtx * 3 + 1]; jz = s_v[vtx * 3 + 2];
-    }
-    s_jo[tid][0] = jx; s_jo[tid][1] = jy; s_jo[tid][2] = jz;
-  }
+  });
+  for (int vtx = tid; vtx < MANO_V; vtx += MANO_THREADS) mano_skin(f, mc.t, vtx, vl);
   __syncthreads();
   if (tid < 21) {
-    int src = mc.new_order[tid];
-    s_jf[tid][0] = s_jo[src][0]; s_jf[tid][1] = s_jo[src][1]; s_jf[tid][2] = s_jo[src][2];
+    const int src = mc.new_order[tid];
+    const float* p = src < 16 ? f.gt[src] : vl + mc.tips[src - 16] * 3;
+    jf[tid][0] = p[0]; jf[tid][1] = p[1]; jf[tid][2] = p[2];
   }
   __syncthreads();
-  if (tid < 3) s_center[tid] = center_idx >= 0 ? s_jf[center_idx][tid] : 0.f;
+  if (tid < 3) center[tid] = center_idx >= 0 ? jf[center_idx][tid] : 0.f;
   __syncthreads();
+}
+
+__global__ void __launch_bounds__(MANO_THREADS)
+mano_fwd_kernel(ManoConsts mc, const float* __restrict__ root_rot, const float* __restrict__ pose, int use_pca, int ncomps,
+                const float* __restrict__ shape, const float* __restrict__ trans, const float* __restrict__ scale,
+                int center_idx, int new_skel, float* __restrict__ v_out, float* __restrict__ j_out) {
+  pdl_sync();
+  __shared__ ManoState f;               // f.vt: v_shaped -> v_tpose -> v_output
+  __shared__ float s_axis[48];
+  __shared__ float s_jf[21][3];         // final joints
+  __shared__ float s_center[3];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  mano_forward(f, s_axis, f.vt, s_jf, s_center, mc, root_rot, pose, use_pca, ncomps, shape, center_idx, b, tid);
   // ---- S6: outputs
   float sc = scale ? scale[b] : 1.f;
   float tr[3] = {0.f, 0.f, 0.f};
   if (trans) { tr[0] = trans[(size_t)b * 3]; tr[1] = trans[(size_t)b * 3 + 1]; tr[2] = trans[(size_t)b * 3 + 2]; }
   for (int o = tid; o < MANO_V3; o += MANO_THREADS) {
     int c = o % 3;
-    float val = s_v[o];
+    float val = f.vt[o];
     if (center_idx >= 0) val = val - s_center[c];
     if (scale) val = val * sc;
     if (trans) val = val + tr[c];
-    s_v[o] = val;
+    f.vt[o] = val;
     v_out[(size_t)b * MANO_V3 + o] = val;
   }
   __syncthreads();
@@ -187,18 +95,18 @@ mano_fwd_kernel(ManoConsts mc, const float* __restrict__ root_rot, const float* 
     if (scale) val = val * sc;
     if (trans) val = val + tr[c];
     if (new_skel) {   // manolayer.py:316-320
-      if (jt == 5) val = (s_v[63 * 3 + c] + s_v[144 * 3 + c]) / 2.f;
-      else if (jt == 9) val = (s_v[271 * 3 + c] + s_v[220 * 3 + c]) / 2.f;
-      else if (jt == 13) val = (s_v[148 * 3 + c] + s_v[290 * 3 + c]) / 2.f;
-      else if (jt == 17) val = (s_v[770 * 3 + c] + s_v[83 * 3 + c]) / 2.f;
+      if (jt == 5) val = (f.vt[63 * 3 + c] + f.vt[144 * 3 + c]) / 2.f;
+      else if (jt == 9) val = (f.vt[271 * 3 + c] + f.vt[220 * 3 + c]) / 2.f;
+      else if (jt == 13) val = (f.vt[148 * 3 + c] + f.vt[290 * 3 + c]) / 2.f;
+      else if (jt == 17) val = (f.vt[770 * 3 + c] + f.vt[83 * 3 + c]) / 2.f;
     }
     j_out[(size_t)b * 63 + tid] = val;
   }
 }
 
 static int fill_consts(ManoConsts& mc, const float* const* const_ptrs, const int* parent, const char* who) {
-  mc.comps = const_ptrs[0]; mc.hands_mean = const_ptrs[1]; mc.shapedirsT = const_ptrs[2]; mc.posedirsT = const_ptrs[3];
-  mc.v_template = const_ptrs[4]; mc.jreg = const_ptrs[5]; mc.weights = const_ptrs[6];
+  mc.comps = const_ptrs[0]; mc.hands_mean = const_ptrs[1];
+  mc.t = ManoTables{const_ptrs[2], const_ptrs[3], const_ptrs[4], const_ptrs[5], const_ptrs[6]};
   for (int i = 0; i < 16; ++i) {
     mc.parent[i] = parent[i];
     RIH_REQUIRE(i == 0 || (parent[i] >= 0 && parent[i] < i), "%s: kinematic parent table is not topologically ordered", who);
@@ -218,21 +126,8 @@ static int fill_consts(ManoConsts& mc, const float* const* const_ptrs, const int
 // resident), then walks the stages in reverse:
 //   B1 outputs -> (trans, scale, centre) gradients, new_skel joints back to their vertex pairs        (block reductions)
 //   B2 joint reorder / finger tips back to vertices
-//   B3 LBS: gG_j = sum_v w[v,j] * (g_v (x) [v_tpose;1])  (warp per joint), g_vtpose = T_v.R^T g_v     (thread per vertex)
-//   B4 FK chain backward, children before parents (one thread; overlaps the per-vertex pass)
-//   B5 pose blend: g_ps[k] = <posedirsT[k], g_vtpose>  (warp per row) ; joint regressor transposed ; shape blend (warp per beta)
+//   B3-B5 mano_backward and mano_shape_row: LBS, FK chain, pose blend, joint regressor and shape blend adjoints
 //   B6 Rodrigues backward (eps added after the norm, manolayer.py:37) and PCA projection
-__device__ __forceinline__ float block_sum_512(float v, float* s_red, int tid) {
-  v = warp_sum(v);
-  __syncthreads();
-  if ((tid & 31) == 0) s_red[tid >> 5] = v;
-  __syncthreads();
-  float t = 0.f;
-#pragma unroll
-  for (int i = 0; i < MANO_THREADS / 32; ++i) t += s_red[i];
-  return t;
-}
-
 __global__ void __launch_bounds__(MANO_THREADS)
 mano_bwd_kernel(ManoConsts mc, const float* __restrict__ root_rot, const float* __restrict__ pose, int use_pca, int ncomps,
                 const float* __restrict__ shape, const float* __restrict__ trans, const float* __restrict__ scale,
@@ -240,140 +135,17 @@ mano_bwd_kernel(ManoConsts mc, const float* __restrict__ root_rot, const float* 
                 float* __restrict__ d_root, float* __restrict__ d_pose, float* __restrict__ d_shape,
                 float* __restrict__ d_trans, float* __restrict__ d_scale) {
   pdl_sync();
-  __shared__ float s_vt[MANO_V3];       // v_shaped -> v_tpose
+  __shared__ ManoState f;               // f.vt: v_shaped -> v_tpose
+  __shared__ ManoGrad gs;
   __shared__ float s_vl[MANO_V3];       // skinned vertices (before centre / scale / trans)
   __shared__ float s_g[MANO_V3];        // gradient buffer: g(v_out) -> g(v_lbs) -> g(v_tpose) -> g(v_shaped)
   __shared__ float s_axis[48];
-  __shared__ float s_R[16][9];
-  __shared__ float s_ps[136];
-  __shared__ float s_beta[10];
-  __shared__ float s_j[16][3];
-  __shared__ float s_t[16][3];          // local translations (I - R_i) j_i
-  __shared__ float s_T[16][12];
-  __shared__ float s_jo[21][3];
   __shared__ float s_jf[21][3];
   __shared__ float s_center[3];
-  __shared__ float s_gjf[21][3], s_gjo[21][3], s_gj[16][3], s_gG[16][12], s_gR[16][9], s_gps[136], s_gaxis[48];
-  __shared__ float s_red[MANO_THREADS / 32];
+  __shared__ float s_gjf[21][3], s_gjo[21][3], s_gaxis[48];
+  __shared__ float s_red[MANO_WARPS];
   const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nwarps = MANO_THREADS / 32;
-
-  // ================= forward recompute (same arithmetic as mano_fwd_kernel)
-  if (tid < 10) s_beta[tid] = shape[(size_t)b * 10 + tid];
-  if (tid < 9) s_R[0][tid] = root_rot[(size_t)b * 9 + tid];
-  __syncthreads();
-  if (use_pca) {
-    if (tid < 45) {
-      float acc = 0.f;
-      for (int i = 0; i < ncomps; ++i) acc = fmaf(pose[(size_t)b * ncomps + i], mc.comps[i * 45 + tid], acc);
-      s_axis[tid] = acc + mc.hands_mean[tid];
-    }
-  } else {
-    if (tid < 135) s_R[1 + tid / 9][tid % 9] = pose[(size_t)b * 135 + tid];
-  }
-  for (int o = tid; o < MANO_V3; o += MANO_THREADS) {
-    float acc = 0.f;
-#pragma unroll
-    for (int i = 0; i < 10; ++i) acc = fmaf(mc.shapedirsT[i * MANO_V3 + o], s_beta[i], acc);
-    s_vt[o] = mc.v_template[o] + acc;
-  }
-  __syncthreads();
-  if (warp == 0) {
-    if (use_pca && lane < 15) {
-      float ax = s_axis[lane * 3], ay = s_axis[lane * 3 + 1], az = s_axis[lane * 3 + 2];
-      float angle = sqrtf(ax * ax + ay * ay + az * az) + 1e-8f;
-      float x = ax / angle, y = ay / angle, z = az / angle;
-      float sn = sinf(angle), cs = cosf(angle), oc = 1.f - cs;
-      float* R = s_R[1 + lane];
-      R[0] = 1.f + oc * (-(z * z) - (y * y)); R[1] = -sn * z + oc * (x * y);        R[2] = sn * y + oc * (x * z);
-      R[3] = sn * z + oc * (x * y);         R[4] = 1.f + oc * (-(z * z) - (x * x)); R[5] = -sn * x + oc * (y * z);
-      R[6] = -sn * y + oc * (x * z);        R[7] = sn * x + oc * (y * z);           R[8] = 1.f + oc * (-(y * y) - (x * x));
-    }
-  } else {
-    for (int o = warp - 1; o < 48; o += nwarps - 1) {
-      int jt = o / 3, c = o % 3;
-      float acc = 0.f;
-      for (int vtx = lane; vtx < MANO_V; vtx += 32) acc = fmaf(mc.jreg[jt * MANO_V + vtx], s_vt[vtx * 3 + c], acc);
-      acc = warp_sum(acc);
-      if (lane == 0) s_j[jt][c] = acc;
-    }
-  }
-  __syncthreads();
-  if (tid < 135) { int k = tid % 9; s_ps[tid] = s_R[1 + tid / 9][k] - ((k == 0 || k == 4 || k == 8) ? 1.f : 0.f); }
-  __syncthreads();
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int i = 0; i < 16; ++i) {
-        const float* R = s_R[i];
-        float jx = s_j[i][0], jy = s_j[i][1], jz = s_j[i][2];
-        float t[3];
-        t[0] = (1.f - R[0]) * jx + (-R[1]) * jy + (-R[2]) * jz;
-        t[1] = (-R[3]) * jx + (1.f - R[4]) * jy + (-R[5]) * jz;
-        t[2] = (-R[6]) * jx + (-R[7]) * jy + (1.f - R[8]) * jz;
-        s_t[i][0] = t[0]; s_t[i][1] = t[1]; s_t[i][2] = t[2];
-        if (i == 0) {
-          for (int r = 0; r < 3; ++r) { s_T[0][r * 4 + 0] = R[r * 3]; s_T[0][r * 4 + 1] = R[r * 3 + 1]; s_T[0][r * 4 + 2] = R[r * 3 + 2]; s_T[0][r * 4 + 3] = t[r]; }
-        } else {
-          const float* P = s_T[mc.parent[i]];
-          for (int r = 0; r < 3; ++r) {
-            float p0 = P[r * 4], p1 = P[r * 4 + 1], p2 = P[r * 4 + 2], p3 = P[r * 4 + 3];
-            s_T[i][r * 4 + 0] = p0 * R[0] + p1 * R[3] + p2 * R[6];
-            s_T[i][r * 4 + 1] = p0 * R[1] + p1 * R[4] + p2 * R[7];
-            s_T[i][r * 4 + 2] = p0 * R[2] + p1 * R[5] + p2 * R[8];
-            s_T[i][r * 4 + 3] = p0 * t[0] + p1 * t[1] + p2 * t[2] + p3;
-          }
-        }
-      }
-    }
-  } else {
-    for (int o = tid - 32; o < MANO_V3; o += MANO_THREADS - 32) {
-      float acc = 0.f;
-#pragma unroll 9
-      for (int i = 0; i < 135; ++i) acc = fmaf(mc.posedirsT[i * MANO_V3 + o], s_ps[i], acc);
-      s_vt[o] += acc;
-    }
-  }
-  __syncthreads();
-  for (int vtx = tid; vtx < MANO_V; vtx += MANO_THREADS) {
-    const float4* w4 = reinterpret_cast<const float4*>(mc.weights + (size_t)vtx * 16);
-    float w[16];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { float4 t = __ldg(w4 + i); w[4 * i] = t.x; w[4 * i + 1] = t.y; w[4 * i + 2] = t.z; w[4 * i + 3] = t.w; }
-    float T[12];
-#pragma unroll
-    for (int e = 0; e < 12; ++e) T[e] = 0.f;
-#pragma unroll
-    for (int jt = 0; jt < 16; ++jt)
-#pragma unroll
-      for (int e = 0; e < 12; ++e) T[e] = fmaf(w[jt], s_T[jt][e], T[e]);
-    float x = s_vt[vtx * 3], y = s_vt[vtx * 3 + 1], z = s_vt[vtx * 3 + 2];
-    s_vl[vtx * 3] = T[0] * x + T[1] * y + T[2] * z + T[3];
-    s_vl[vtx * 3 + 1] = T[4] * x + T[5] * y + T[6] * z + T[7];
-    s_vl[vtx * 3 + 2] = T[8] * x + T[9] * y + T[10] * z + T[11];
-  }
-  __syncthreads();
-  if (tid < 21) {
-    float jx, jy, jz;
-    if (tid == 0) { jx = s_j[0][0]; jy = s_j[0][1]; jz = s_j[0][2]; }
-    else if (tid < 16) {
-      const float* P = s_T[mc.parent[tid]];
-      float x = s_j[tid][0], y = s_j[tid][1], z = s_j[tid][2];
-      jx = P[0] * x + P[1] * y + P[2] * z + P[3];
-      jy = P[4] * x + P[5] * y + P[6] * z + P[7];
-      jz = P[8] * x + P[9] * y + P[10] * z + P[11];
-    } else {
-      int vtx = mc.tips[tid - 16];
-      jx = s_vl[vtx * 3]; jy = s_vl[vtx * 3 + 1]; jz = s_vl[vtx * 3 + 2];
-    }
-    s_jo[tid][0] = jx; s_jo[tid][1] = jy; s_jo[tid][2] = jz;
-  }
-  __syncthreads();
-  if (tid < 21) {
-    int src = mc.new_order[tid];
-    s_jf[tid][0] = s_jo[src][0]; s_jf[tid][1] = s_jo[src][1]; s_jf[tid][2] = s_jo[src][2];
-  }
-  __syncthreads();
-  if (tid < 3) s_center[tid] = center_idx >= 0 ? s_jf[center_idx][tid] : 0.f;
+  mano_forward(f, s_axis, s_vl, s_jf, s_center, mc, root_rot, pose, use_pca, ncomps, shape, center_idx, b, tid);
 
   // ================= B1: output affine (centre / scale / trans) and new_skel
   for (int o = tid; o < MANO_V3; o += MANO_THREADS) s_g[o] = g_v ? g_v[(size_t)b * MANO_V3 + o] : 0.f;
@@ -404,8 +176,8 @@ mano_bwd_kernel(ManoConsts mc, const float* __restrict__ root_rot, const float* 
     p0 += gx; p1 += gy; p2 += gz;
     ps += gx * (s_jf[tid][0] - s_center[0]) + gy * (s_jf[tid][1] - s_center[1]) + gz * (s_jf[tid][2] - s_center[2]);
   }
-  const float sum0 = block_sum_512(p0, s_red, tid), sum1 = block_sum_512(p1, s_red, tid), sum2 = block_sum_512(p2, s_red, tid);
-  const float sums = block_sum_512(ps, s_red, tid);
+  const float sum0 = block_sum<MANO_WARPS>(p0, s_red, tid), sum1 = block_sum<MANO_WARPS>(p1, s_red, tid);
+  const float sum2 = block_sum<MANO_WARPS>(p2, s_red, tid), sums = block_sum<MANO_WARPS>(ps, s_red, tid);
   if (tid == 0) {
     if (d_trans) { d_trans[(size_t)b * 3] = trans ? sum0 : 0.f; d_trans[(size_t)b * 3 + 1] = trans ? sum1 : 0.f; d_trans[(size_t)b * 3 + 2] = trans ? sum2 : 0.f; }
     if (d_scale) d_scale[b] = scale ? sums : 0.f;
@@ -421,126 +193,16 @@ mano_bwd_kernel(ManoConsts mc, const float* __restrict__ root_rot, const float* 
   __syncthreads();
   if (tid < 15) s_g[mc.tips[tid / 3] * 3 + tid % 3] += s_gjo[16 + tid / 3][tid % 3];
   __syncthreads();
-  // ================= B3a: gG_j from the skinning (warp j <-> joint j; 16 warps)
-  {
-    const int jt = warp;
-    float a[12];
-#pragma unroll
-    for (int e = 0; e < 12; ++e) a[e] = 0.f;
-    for (int vtx = lane; vtx < MANO_V; vtx += 32) {
-      const float w = __ldg(mc.weights + (size_t)vtx * 16 + jt);
-      const float gx = w * s_g[vtx * 3], gy = w * s_g[vtx * 3 + 1], gz = w * s_g[vtx * 3 + 2];
-      const float x = s_vt[vtx * 3], y = s_vt[vtx * 3 + 1], z = s_vt[vtx * 3 + 2];
-      a[0] = fmaf(gx, x, a[0]); a[1] = fmaf(gx, y, a[1]); a[2] = fmaf(gx, z, a[2]); a[3] += gx;
-      a[4] = fmaf(gy, x, a[4]); a[5] = fmaf(gy, y, a[5]); a[6] = fmaf(gy, z, a[6]); a[7] += gy;
-      a[8] = fmaf(gz, x, a[8]); a[9] = fmaf(gz, y, a[9]); a[10] = fmaf(gz, z, a[10]); a[11] += gz;
-    }
-#pragma unroll
-    for (int e = 0; e < 12; ++e) { a[e] = warp_sum(a[e]); }
-    if (lane == 0) {
-#pragma unroll
-      for (int e = 0; e < 12; ++e) s_gG[jt][e] = a[e];
-    }
-  }
-  __syncthreads();
-  // ================= B3b (warps 1..) g_vtpose = T_v.R^T g_v   ||   B4 (thread 0) joints + FK chain backward
-  if (warp == 0) {
-    if (lane == 0) {
-      // joints: jo[0] = j[0]; jo[i] = G_parent(i).R j_i + G_parent(i).t
-      s_gj[0][0] = s_gjo[0][0]; s_gj[0][1] = s_gjo[0][1]; s_gj[0][2] = s_gjo[0][2];
-      for (int i = 1; i < 16; ++i) {
-        const int p = mc.parent[i];
-        const float* P = s_T[p];
-        const float g0 = s_gjo[i][0], g1 = s_gjo[i][1], g2 = s_gjo[i][2];
-        s_gj[i][0] = P[0] * g0 + P[4] * g1 + P[8] * g2;
-        s_gj[i][1] = P[1] * g0 + P[5] * g1 + P[9] * g2;
-        s_gj[i][2] = P[2] * g0 + P[6] * g1 + P[10] * g2;
-        const float g[3] = {g0, g1, g2};
-        for (int r = 0; r < 3; ++r) {
-          s_gG[p][r * 4 + 0] += g[r] * s_j[i][0]; s_gG[p][r * 4 + 1] += g[r] * s_j[i][1]; s_gG[p][r * 4 + 2] += g[r] * s_j[i][2];
-          s_gG[p][r * 4 + 3] += g[r];
-        }
-      }
-      // chain: G_i.R = G_p.R R_i ; G_i.t = G_p.R t_i + G_p.t   (children carry larger indices than their parents)
-      for (int i = 15; i >= 0; --i) {
-        const float* gG = s_gG[i];
-        const float* R = s_R[i];
-        float gR[9], gt[3];
-        if (i > 0) {
-          const int p = mc.parent[i];
-          const float* P = s_T[p];
-          float* gP = s_gG[p];
-          for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c)
-              gP[r * 4 + c] += gG[r * 4 + 0] * R[c * 3 + 0] + gG[r * 4 + 1] * R[c * 3 + 1] + gG[r * 4 + 2] * R[c * 3 + 2] + gG[r * 4 + 3] * s_t[i][c];
-            gP[r * 4 + 3] += gG[r * 4 + 3];
-          }
-          for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c) gR[r * 3 + c] = P[0 * 4 + r] * gG[0 * 4 + c] + P[1 * 4 + r] * gG[1 * 4 + c] + P[2 * 4 + r] * gG[2 * 4 + c];
-            gt[r] = P[0 * 4 + r] * gG[3] + P[1 * 4 + r] * gG[7] + P[2 * 4 + r] * gG[11];
-          }
-        } else {
-          for (int r = 0; r < 3; ++r) { gR[r * 3] = gG[r * 4]; gR[r * 3 + 1] = gG[r * 4 + 1]; gR[r * 3 + 2] = gG[r * 4 + 2]; gt[r] = gG[r * 4 + 3]; }
-        }
-        // t_i = (I - R_i) j_i
-        for (int c = 0; c < 3; ++c) s_gj[i][c] += gt[c] - (R[0 * 3 + c] * gt[0] + R[1 * 3 + c] * gt[1] + R[2 * 3 + c] * gt[2]);
-        for (int r = 0; r < 3; ++r)
-          for (int c = 0; c < 3; ++c) s_gR[i][r * 3 + c] = gR[r * 3 + c] - gt[r] * s_j[i][c];
-      }
-    }
-  } else {
-    for (int vtx = tid - 32; vtx < MANO_V; vtx += MANO_THREADS - 32) {
-      const float4* w4 = reinterpret_cast<const float4*>(mc.weights + (size_t)vtx * 16);
-      float w[16];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) { float4 t = __ldg(w4 + i); w[4 * i] = t.x; w[4 * i + 1] = t.y; w[4 * i + 2] = t.z; w[4 * i + 3] = t.w; }
-      float T[9];
-#pragma unroll
-      for (int e = 0; e < 9; ++e) T[e] = 0.f;
-#pragma unroll
-      for (int jt = 0; jt < 16; ++jt)
-#pragma unroll
-        for (int r = 0; r < 3; ++r)
-#pragma unroll
-          for (int c = 0; c < 3; ++c) T[r * 3 + c] = fmaf(w[jt], s_T[jt][r * 4 + c], T[r * 3 + c]);
-      const float gx = s_g[vtx * 3], gy = s_g[vtx * 3 + 1], gz = s_g[vtx * 3 + 2];
-      s_g[vtx * 3] = T[0] * gx + T[3] * gy + T[6] * gz;
-      s_g[vtx * 3 + 1] = T[1] * gx + T[4] * gy + T[7] * gz;
-      s_g[vtx * 3 + 2] = T[2] * gx + T[5] * gy + T[8] * gz;
-    }
-  }
-  __syncthreads();
-  // ================= B5a: pose blend rows (warp per k), then into gR
-  for (int k = warp; k < 135; k += nwarps) {
-    float acc = 0.f;
-    const float* row = mc.posedirsT + (size_t)k * MANO_V3;
-    for (int o = lane; o < MANO_V3; o += 32) acc = fmaf(__ldg(row + o), s_g[o], acc);
-    acc = warp_sum(acc);
-    if (lane == 0) s_gps[k] = acc;
-  }
-  __syncthreads();
-  if (tid < 135) s_gR[1 + tid / 9][tid % 9] += s_gps[tid];
-  // ================= B5b: joint regressor transposed: g_vshaped = g_vtpose + Jreg^T g_j
-  for (int o = tid; o < MANO_V3; o += MANO_THREADS) {
-    const int vtx = o / 3, c = o - vtx * 3;
-    float acc = s_g[o];
-#pragma unroll
-    for (int jt = 0; jt < 16; ++jt) acc = fmaf(__ldg(mc.jreg + jt * MANO_V + vtx), s_gj[jt][c], acc);
-    s_g[o] = acc;
-  }
-  __syncthreads();
+  // ================= B3-B5
+  mano_backward(f, mc.t, mc.parent, s_g, s_gjo, nullptr, gs, tid);
   // ================= B5c: shape blend (warps 0..9) || B6: rotations (warp 10)
   if (warp < 10) {
-    float acc = 0.f;
-    const float* row = mc.shapedirsT + (size_t)warp * MANO_V3;
-    for (int o = lane; o < MANO_V3; o += 32) acc = fmaf(__ldg(row + o), s_g[o], acc);
-    acc = warp_sum(acc);
-    if (lane == 0 && d_shape) d_shape[(size_t)b * 10 + warp] = acc;
+    if (d_shape) mano_shape_row(mc.t, s_g, warp, lane, d_shape + (size_t)b * 10 + warp);
   } else if (warp == 10) {
-    if (d_root && lane < 9) d_root[(size_t)b * 9 + lane] = s_gR[0][lane];
+    if (d_root && lane < 9) d_root[(size_t)b * 9 + lane] = gs.gR[0][lane];
     if (d_pose) {
       if (!use_pca) {
-        for (int i = lane; i < 135; i += 32) d_pose[(size_t)b * 135 + i] = s_gR[1 + i / 9][i % 9];
+        for (int i = lane; i < 135; i += 32) d_pose[(size_t)b * 135 + i] = gs.gR[1 + i / 9][i % 9];
       } else {
         if (lane < 15) {
           const float ax = s_axis[lane * 3], ay = s_axis[lane * 3 + 1], az = s_axis[lane * 3 + 2];
@@ -548,7 +210,7 @@ mano_bwd_kernel(ManoConsts mc, const float* __restrict__ root_rot, const float* 
           const float th = nrm + 1e-8f;
           const float x = ax / th, y = ay / th, z = az / th;
           const float sn = sinf(th), cs = cosf(th), oc = 1.f - cs;
-          const float* g = s_gR[1 + lane];
+          const float* g = gs.gR[1 + lane];
           const float gx = -2.f * oc * x * (g[4] + g[8]) + oc * y * (g[1] + g[3]) + oc * z * (g[2] + g[6]) + sn * (g[7] - g[5]);
           const float gy = -2.f * oc * y * (g[0] + g[8]) + oc * x * (g[1] + g[3]) + oc * z * (g[5] + g[7]) + sn * (g[2] - g[6]);
           const float gz = -2.f * oc * z * (g[0] + g[4]) + oc * x * (g[2] + g[6]) + oc * y * (g[5] + g[7]) + sn * (g[3] - g[1]);
